@@ -42,6 +42,13 @@ enum {
     BMPC_UNSOLVED = -10
 };
 
+/* per-instance status written by bmpc_dare */
+enum {
+    BMPC_DARE_SOLVED = 1,       /* stabilising solution: X converged and the closed-loop powers decayed */
+    BMPC_DARE_NO_SOLUTION = -1, /* no stabilising solution (64 doubling steps without convergence and decay, or a non-finite iterate) */
+    BMPC_DARE_R_NOT_PD = -2     /* R is not positive definite */
+};
+
 typedef struct {
     int32_t nx, nu, Np, Nc;     /* Nc <= 0 means Nc = Np            (mpc.py:76-108) */
     int32_t batch;              /* instances on this device */
@@ -144,8 +151,13 @@ int bmpc_get_dims(const bmpc_handle* h, int32_t* dims);
  * The state lives on the device; bmpc_est_state_ptr() can be handed to bmpc_update(..., on_device=1) so the whole
  * control loop (estimate -> MPC -> plant input) stays on the GPU. */
 typedef struct bmpc_estimator bmpc_estimator;
+/* one (A,B,C,L) shared by every instance: bmpc_est_create_ex(..., n_sys = 1, ...) */
 int bmpc_est_create(int32_t nx, int32_t nu, int32_t ny, int32_t batch, int32_t device, const double* A, const double* B,
                     const double* C, const double* L, const double* x0 /* [batch,nx] host */, bmpc_estimator** out);
+/* n_sys = 1: shared (A,B,C,L); n_sys = batch: one system per instance, each array with a leading batch dimension (host pointers,
+ * batch-major, row-major).  Per-instance systems run one thread per instance with the matrices in global memory. */
+int bmpc_est_create_ex(int32_t nx, int32_t nu, int32_t ny, int32_t batch, int32_t n_sys, int32_t device, const double* A,
+                       const double* B, const double* C, const double* L, const double* x0, bmpc_estimator** out);
 void bmpc_est_destroy(bmpc_estimator* e);
 int bmpc_est_predict(bmpc_estimator* e, const double* u /* [batch,nu] */, int on_device);
 int bmpc_est_update(bmpc_estimator* e, const double* y_meas /* [batch,ny] */, int on_device);
@@ -156,6 +168,15 @@ int bmpc_est_set_stream(bmpc_estimator* e, void* cuda_stream);
  * kernels are ordered against bmpc_update(on_device=1) reading bmpc_est_state_ptr() and against the solver writing u0), and
  * a predict/update that takes a device pointer first retires the controller's deferred solve.  h = NULL detaches. */
 int bmpc_est_attach(bmpc_estimator* e, bmpc_handle* h);
+
+/* ---- batched DARE, the design step of kalman_design / kalman_design_simple (kalman.py:67, 96: control.dare):
+ *   X = A'XA - (A'XB + S)(R + B'XB)^-1 (B'XA + S') + Q,   G = (R + B'XB)^-1 (B'XA + S')
+ * for `batch` independent instances, 1 <= n, m <= 32, by structured doubling in fp64 (csrc/bmpc_dare.cuh).
+ * A [batch,n,n], B [batch,n,m], Q [batch,n,n], R [batch,m,m], S [batch,n,m] (NULL: no cross term) in; X [batch,n,n],
+ * G [batch,m,n], status [batch] (BMPC_DARE_*), iters [batch] (doubling steps) out.  Host pointers; synchronises before it returns.
+ * X and G of an instance with status < 0 are NaN. */
+int bmpc_dare(int32_t n, int32_t m, int32_t batch, int32_t device, const double* A, const double* B, const double* Q,
+              const double* R, const double* S, double* X, double* G, int32_t* status, int32_t* iters);
 
 /* pinned host memory for the end-to-end path (cudaHostAlloc mapped + portable / cudaFreeHost): the GPU can read and write it in place,
  * so such a buffer may be passed to bmpc_update(..., on_device = 2) and to bmpc_bind_output — the solver kernels then fetch x0 / u_-1

@@ -31,8 +31,8 @@ EXPORTS = ["bmpc_default_config", "bmpc_create", "bmpc_destroy", "bmpc_last_erro
            "bmpc_solve", "bmpc_output", "bmpc_get_sequences", "bmpc_bind_output", "bmpc_bind_output_peers", "bmpc_bind_gather_flags",
            "bmpc_gather_arrive", "bmpc_set_stream",
            "bmpc_synchronize", "bmpc_get_stats", "bmpc_get_sys", "bmpc_get_dims", "bmpc_host_alloc",
-           "bmpc_host_free", "bmpc_device_count", "bmpc_has_fast_path", "bmpc_has_multi_input_fast_path", "bmpc_est_create", "bmpc_est_destroy", "bmpc_est_predict",
-           "bmpc_est_update", "bmpc_est_get", "bmpc_est_state_ptr", "bmpc_est_set_stream", "bmpc_est_attach"]
+           "bmpc_host_free", "bmpc_device_count", "bmpc_has_fast_path", "bmpc_has_multi_input_fast_path", "bmpc_est_create", "bmpc_est_create_ex", "bmpc_est_destroy", "bmpc_est_predict",
+           "bmpc_est_update", "bmpc_est_get", "bmpc_est_state_ptr", "bmpc_est_set_stream", "bmpc_est_attach", "bmpc_dare"]
 
 
 class BmpcError(RuntimeError):
@@ -75,6 +75,7 @@ def load(path=None):
     L.bmpc_host_free.argtypes = [P]; L.bmpc_host_free.restype = None
     L.bmpc_device_count.argtypes = []; L.bmpc_device_count.restype = ctypes.c_int
     L.bmpc_est_create.argtypes = [ctypes.c_int32] * 5 + [DP] * 5 + [ctypes.POINTER(P)]; L.bmpc_est_create.restype = ctypes.c_int
+    L.bmpc_est_create_ex.argtypes = [ctypes.c_int32] * 6 + [DP] * 5 + [ctypes.POINTER(P)]; L.bmpc_est_create_ex.restype = ctypes.c_int
     L.bmpc_est_destroy.argtypes = [P]; L.bmpc_est_destroy.restype = None
     L.bmpc_est_predict.argtypes = [P, DP, ctypes.c_int]; L.bmpc_est_predict.restype = ctypes.c_int
     L.bmpc_est_update.argtypes = [P, DP, ctypes.c_int]; L.bmpc_est_update.restype = ctypes.c_int
@@ -82,6 +83,7 @@ def load(path=None):
     L.bmpc_est_state_ptr.argtypes = [P]; L.bmpc_est_state_ptr.restype = P
     L.bmpc_est_set_stream.argtypes = [P, P]; L.bmpc_est_set_stream.restype = ctypes.c_int
     L.bmpc_est_attach.argtypes = [P, P]; L.bmpc_est_attach.restype = ctypes.c_int
+    L.bmpc_dare.argtypes = [ctypes.c_int32] * 4 + [DP] * 9; L.bmpc_dare.restype = ctypes.c_int
     L.bmpc_has_fast_path.argtypes = [ctypes.c_int] * 4; L.bmpc_has_fast_path.restype = ctypes.c_int
     L.bmpc_has_multi_input_fast_path.argtypes = [ctypes.c_int] * 4; L.bmpc_has_multi_input_fast_path.restype = ctypes.c_int
     _libs[path] = L

@@ -20,6 +20,7 @@
 #include "bmpc_tpi.cuh"
 #include "bmpc_tile.cuh"
 #include "bmpc_tpm.cuh"
+#include "bmpc_dare.cuh"
 
 // One block of round counters = BMPC_CNT ints (the handle keeps two, used alternately): [0] instances still unfinished (-> next list),
 // [1] active-set refinements, [2] overflow of the small polish tier, [3] certified infeasible, [4..7] queue control of k_tpi_pol
@@ -1915,8 +1916,55 @@ __global__ void k_est(int nx, int nu, int ny, int B, const double* __restrict__ 
     }
 }
 
+// the same estimator with one (A, B, C, L) per instance: matrices in global memory, FIELD-major (element e of instance b at
+// mats[e * B + b]) so that the 32 threads of a warp read 32 consecutive doubles; same operation order as k_est
+__global__ void k_est_pi(int nx, int nu, int ny, int B, const double* __restrict__ mats, double* __restrict__ x, double* __restrict__ y,
+                         const double* __restrict__ in, int mode) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= B) return;
+    const double *A = mats + b, *Bm = A + (size_t)nx * nx * B, *C = Bm + (size_t)nx * nu * B, *L = C + (size_t)ny * nx * B;
+    double* xb = x + (size_t)b * nx; double* yb = y + (size_t)b * ny;
+    double xn[32];
+    if (mode == 0) {            // predict: x <- A x + B u ; y <- C x
+        const double* u = in + (size_t)b * nu;
+        for (int i = 0; i < nx; i++) {
+            double acc = 0.0;
+            for (int j = 0; j < nx; j++) acc += A[(size_t)(i * nx + j) * B] * xb[j];
+            for (int j = 0; j < nu; j++) acc += Bm[(size_t)(i * nu + j) * B] * u[j];
+            xn[i] = acc;
+        }
+        for (int i = 0; i < nx; i++) xb[i] = xn[i];
+        for (int i = 0; i < ny; i++) { double acc = 0.0; for (int j = 0; j < nx; j++) acc += C[(size_t)(i * nx + j) * B] * xn[j]; yb[i] = acc; }
+    } else {                    // update: x <- x + L (y_meas - y)      (y is NOT refreshed, as in the reference)
+        const double* ym = in + (size_t)b * ny;
+        for (int i = 0; i < nx; i++) {
+            double acc = xb[i];
+            for (int j = 0; j < ny; j++) acc += L[(size_t)(i * ny + j) * B] * (ym[j] - yb[j]);
+            xn[i] = acc;
+        }
+        for (int i = 0; i < nx; i++) xb[i] = xn[i];
+    }
+}
+
+// batched DARE (csrc/bmpc_dare.cuh): one warp per instance, lane = row, the iterates in dynamic shared memory
+__global__ void k_dare(int n, int m, int batch, const double* __restrict__ A, const double* __restrict__ B, const double* __restrict__ Q,
+                       const double* __restrict__ R, const double* S, double* __restrict__ X, double* __restrict__ G,
+                       int* __restrict__ status, int* __restrict__ steps) {
+    extern __shared__ double sm[];
+    const BmpcDareLayout l = bmpc_dare_layout(n, m);
+    const int w = threadIdx.x >> 5;
+    const int b = blockIdx.x * (blockDim.x >> 5) + w;
+    if (b >= batch) return;                                  // whole warps leave: the team below always has 32 lanes
+    WarpTeam t;
+    const size_t nn = (size_t)n * n, nm = (size_t)n * m;
+    int it = 0;
+    const int st = bmpc_dare_solve(t, n, m, l, A + b * nn, B + b * nm, Q + b * nn, R + (size_t)b * m * m, S ? S + b * nm : nullptr,
+                                   X + b * nn, G + b * nm, sm + (size_t)w * l.total, it);
+    if (t.tid == 0) { status[b] = st; steps[b] = it; }
+}
+
 struct bmpc_estimator {
-    int nx, nu, ny, B, device;
+    int nx, nu, ny, B, device, n_sys;
     double *mats = nullptr, *x = nullptr, *y = nullptr, *in = nullptr;
     cudaStream_t stream = nullptr, own = nullptr;
     bmpc_handle* mpc = nullptr;        // attached controller: same stream, and its deferred solve is retired before its u0 is read
@@ -1926,27 +1974,44 @@ extern "C" {
 
 int bmpc_est_create(int32_t nx, int32_t nu, int32_t ny, int32_t batch, int32_t device, const double* A, const double* B,
                     const double* C, const double* L, const double* x0, bmpc_estimator** out) {
+    return bmpc_est_create_ex(nx, nu, ny, batch, 1, device, A, B, C, L, x0, out);
+}
+
+int bmpc_est_create_ex(int32_t nx, int32_t nu, int32_t ny, int32_t batch, int32_t n_sys, int32_t device, const double* A, const double* B,
+                       const double* C, const double* L, const double* x0, bmpc_estimator** out) {
     if (!out || !A || !B || !C || !L || !x0 || nx < 1 || nx > 32 || nu < 1 || ny < 1 || batch < 1) { g_create_err = "bmpc_est_create: bad argument (1 <= nx <= 32)"; return BMPC_ERR_ARG; }
+    if (n_sys != 1 && n_sys != batch) { g_create_err = "bmpc_est_create: n_sys must be 1 (shared system) or batch (one system per instance)"; return BMPC_ERR_ARG; }
     *out = nullptr;
     if (bmpc_device_count() <= device) { g_create_err = "no CUDA device visible: libbmpc has no CPU fallback"; return BMPC_ERR_NO_DEVICE; }
     cudaSetDevice(device);
     bmpc_estimator* e = new bmpc_estimator();
-    e->nx = nx; e->nu = nu; e->ny = ny; e->B = batch; e->device = device;
+    e->nx = nx; e->nu = nu; e->ny = ny; e->B = batch; e->device = device; e->n_sys = n_sys;
     const size_t nm = (size_t)nx * nx + (size_t)nx * nu + (size_t)ny * nx + (size_t)nx * ny;
     const int mx = nu > ny ? nu : ny;
-    bool ok = cudaMalloc((void**)&e->mats, nm * 8) == cudaSuccess && cudaMalloc((void**)&e->x, (size_t)batch * nx * 8) == cudaSuccess &&
+    bool ok = cudaMalloc((void**)&e->mats, nm * n_sys * 8) == cudaSuccess && cudaMalloc((void**)&e->x, (size_t)batch * nx * 8) == cudaSuccess &&
               cudaMalloc((void**)&e->y, (size_t)batch * ny * 8) == cudaSuccess && cudaMalloc((void**)&e->in, (size_t)batch * mx * 8) == cudaSuccess &&
               cudaStreamCreateWithFlags(&e->own, cudaStreamNonBlocking) == cudaSuccess;
     if (!ok) { g_create_err = "bmpc_est_create: allocation failed"; bmpc_est_destroy(e); return BMPC_ERR_CUDA; }
     e->stream = e->own;
-    std::vector<double> m(nm);
-    memcpy(m.data(), A, sizeof(double) * nx * nx); memcpy(m.data() + nx * nx, B, sizeof(double) * nx * nu);
-    memcpy(m.data() + nx * nx + nx * nu, C, sizeof(double) * ny * nx); memcpy(m.data() + nx * nx + nx * nu + ny * nx, L, sizeof(double) * nx * ny);
-    cudaMemcpyAsync(e->mats, m.data(), nm * 8, cudaMemcpyHostToDevice, e->stream);
+    // packed (A, B, C, L) of each system; with n_sys = batch transposed to field-major for k_est_pi
+    const size_t cnt[4] = {(size_t)nx * nx, (size_t)nx * nu, (size_t)ny * nx, (size_t)nx * ny};
+    const double* src[4] = {A, B, C, L};
+    std::vector<double> m(nm * n_sys);
+    for (int s = 0; s < n_sys; s++) {
+        size_t e0 = 0;
+        for (int f = 0; f < 4; f++) {
+            for (size_t k = 0; k < cnt[f]; k++) m[(e0 + k) * n_sys + s] = src[f][s * cnt[f] + k];
+            e0 += cnt[f];
+        }
+    }
+    cudaMemcpyAsync(e->mats, m.data(), m.size() * 8, cudaMemcpyHostToDevice, e->stream);
     cudaMemcpyAsync(e->x, x0, (size_t)batch * nx * 8, cudaMemcpyHostToDevice, e->stream);
     // y = C x0 (kalman.py:113): a predict with A = I, B = 0 would do; compute on the host instead (setup only)
     std::vector<double> y0((size_t)batch * ny);
-    for (int b = 0; b < batch; b++) for (int i = 0; i < ny; i++) { double acc = 0; for (int j = 0; j < nx; j++) acc += C[i * nx + j] * x0[(size_t)b * nx + j]; y0[(size_t)b * ny + i] = acc; }
+    for (int b = 0; b < batch; b++) {
+        const double* Cb = C + (n_sys == 1 ? 0 : (size_t)b * ny * nx);
+        for (int i = 0; i < ny; i++) { double acc = 0; for (int j = 0; j < nx; j++) acc += Cb[i * nx + j] * x0[(size_t)b * nx + j]; y0[(size_t)b * ny + i] = acc; }
+    }
     cudaMemcpyAsync(e->y, y0.data(), y0.size() * 8, cudaMemcpyHostToDevice, e->stream);
     if (cudaStreamSynchronize(e->stream) != cudaSuccess) { g_create_err = "bmpc_est_create: upload failed"; bmpc_est_destroy(e); return BMPC_ERR_CUDA; }
     *out = e;
@@ -1976,7 +2041,10 @@ static int est_run(bmpc_estimator* e, const double* in, int n, int on_device, in
         src = e->in;
     }
     const size_t nm = (size_t)e->nx * e->nx + (size_t)e->nx * e->nu + (size_t)e->ny * e->nx + (size_t)e->nx * e->ny;
-    k_est<<<(e->B + 127) / 128, 128, nm * 8, e->stream>>>(e->nx, e->nu, e->ny, e->B, e->mats, e->x, e->y, src, mode);
+    if (e->n_sys == 1)
+        k_est<<<(e->B + 127) / 128, 128, nm * 8, e->stream>>>(e->nx, e->nu, e->ny, e->B, e->mats, e->x, e->y, src, mode);
+    else
+        k_est_pi<<<(e->B + 127) / 128, 128, 0, e->stream>>>(e->nx, e->nu, e->ny, e->B, e->mats, e->x, e->y, src, mode);
     return cudaGetLastError() == cudaSuccess ? BMPC_OK : BMPC_ERR_CUDA;
 }
 int bmpc_est_predict(bmpc_estimator* e, const double* u, int on_device) { return est_run(e, u, e ? e->nu : 0, on_device, 0); }
@@ -1995,6 +2063,55 @@ int bmpc_est_attach(bmpc_estimator* e, bmpc_handle* h) {
     if (h && h->cfg.device != e->device) return BMPC_ERR_ARG;
     cudaSetDevice(e->device); cudaStreamSynchronize(e->stream);
     e->mpc = h; e->stream = h ? h->stream : e->own;
+    return BMPC_OK;
+}
+
+int bmpc_dare(int32_t n, int32_t m, int32_t batch, int32_t device, const double* A, const double* B, const double* Q,
+              const double* R, const double* S, double* X, double* G, int32_t* status, int32_t* iters) {
+    if (!A || !B || !Q || !R || !X || !G || !status || !iters || n < 1 || n > BMPC_DARE_MAX_DIM || m < 1 || m > BMPC_DARE_MAX_DIM || batch < 1) {
+        g_create_err = "bmpc_dare: bad argument (1 <= n, m <= 32, batch >= 1)"; return BMPC_ERR_ARG;
+    }
+    if (device < 0 || bmpc_device_count() <= device) { g_create_err = "no CUDA device visible: libbmpc has no CPU fallback"; return BMPC_ERR_NO_DEVICE; }
+    if (cudaSetDevice(device) != cudaSuccess) { g_create_err = "bmpc_dare: cudaSetDevice failed"; return BMPC_ERR_CUDA; }
+    const BmpcDareLayout l = bmpc_dare_layout(n, m);
+    int optin = 0;
+    cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device);
+    const size_t per_warp = (size_t)l.total * 8;
+    int wpb = (int)((size_t)optin / per_warp);
+    if (wpb > 8) wpb = 8;
+    if (wpb > batch) wpb = batch;
+    if (wpb < 1) { g_create_err = "bmpc_dare: workspace exceeds the shared memory of one block"; return BMPC_ERR_ARG; }
+    const size_t smem = per_warp * wpb;
+    if (smem > 48 * 1024 && cudaFuncSetAttribute(k_dare, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
+        g_create_err = "bmpc_dare: cannot raise the dynamic shared memory limit"; return BMPC_ERR_CUDA;
+    }
+    const size_t b = (size_t)batch, nn = (size_t)n * n, nm = (size_t)n * m, mm = (size_t)m * m;
+    const size_t nd = b * (3 * nn + 3 * nm + mm);                  // A, Q, X | B, S, G | R
+    cudaStream_t s = nullptr;
+    if (cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking) != cudaSuccess) { g_create_err = "bmpc_dare: stream creation failed"; return BMPC_ERR_CUDA; }
+    double* d = nullptr;
+    if (cudaMallocAsync((void**)&d, nd * 8 + b * 8, s) != cudaSuccess) {
+        cudaStreamDestroy(s); g_create_err = "bmpc_dare: allocation failed"; return BMPC_ERR_CUDA;
+    }
+    double *dA = d, *dQ = dA + b * nn, *dX = dQ + b * nn, *dB = dX + b * nn, *dS = dB + b * nm, *dG = dS + b * nm, *dR = dG + b * nm;
+    int* dst = (int*)(dR + b * mm); int* dit = dst + b;
+    bool ok = cudaMemcpyAsync(dA, A, b * nn * 8, cudaMemcpyHostToDevice, s) == cudaSuccess &&
+              cudaMemcpyAsync(dQ, Q, b * nn * 8, cudaMemcpyHostToDevice, s) == cudaSuccess &&
+              cudaMemcpyAsync(dB, B, b * nm * 8, cudaMemcpyHostToDevice, s) == cudaSuccess &&
+              cudaMemcpyAsync(dR, R, b * mm * 8, cudaMemcpyHostToDevice, s) == cudaSuccess &&
+              (!S || cudaMemcpyAsync(dS, S, b * nm * 8, cudaMemcpyHostToDevice, s) == cudaSuccess);
+    if (ok) {
+        k_dare<<<(batch + wpb - 1) / wpb, 32 * wpb, smem, s>>>(n, m, batch, dA, dB, dQ, dR, S ? dS : nullptr, dX, dG, dst, dit);
+        ok = cudaGetLastError() == cudaSuccess &&
+             cudaMemcpyAsync(X, dX, b * nn * 8, cudaMemcpyDeviceToHost, s) == cudaSuccess &&
+             cudaMemcpyAsync(G, dG, b * nm * 8, cudaMemcpyDeviceToHost, s) == cudaSuccess &&
+             cudaMemcpyAsync(status, dst, b * 4, cudaMemcpyDeviceToHost, s) == cudaSuccess &&
+             cudaMemcpyAsync(iters, dit, b * 4, cudaMemcpyDeviceToHost, s) == cudaSuccess;
+    }
+    cudaFreeAsync(d, s);
+    ok = cudaStreamSynchronize(s) == cudaSuccess && ok;
+    cudaStreamDestroy(s);
+    if (!ok) { g_create_err = std::string("bmpc_dare: ") + cudaGetErrorString(cudaGetLastError()); return BMPC_ERR_CUDA; }
     return BMPC_OK;
 }
 

@@ -1,11 +1,16 @@
-"""Batched ``LinearStateEstimator`` on the GPU — the step on the input side of the MPC path (SURVEY.md §8f-4).
+"""Kalman design and the batched ``LinearStateEstimator`` on the GPU — the input side of the MPC path (SURVEY.md §8f-4).
 
-Mirrors ``/root/reference/pyMPC/kalman.py:109-152`` (``__init__``, ``out_y``, ``predict``, ``update``, ``sim``) for a
-batch of B estimators that share (A, B, C, D, L): ``predict(u)`` does ``x <- A x + B u; y <- C x`` (kalman.py:126-129)
-and ``update(y_meas)`` does ``x <- x + L (y_meas - y)`` (kalman.py:131-133, ``y`` is not refreshed — as in the
-reference).  The state stays on the device; ``device_state()`` feeds ``MPCController.update_from_device``.
-The Kalman *design* helpers (``kalman_design*``: DARE through the ``control`` package, kalman.py:24-106) are out of
-scope: they run once, on the host, and produce the gain ``L`` this class takes.
+Mirrors ``/root/reference/pyMPC/kalman.py``:
+
+* ``dare`` replaces the ``control.dare`` calls of the reference (kalman.py:67, 96); ``kalman_design`` (kalman.py:24-70) and
+  ``kalman_design_simple`` (kalman.py:73-106) follow the reference's formulas on top of it.  The Riccati equations are solved on
+  the device (``bmpc_dare``: structured doubling, one warp per instance), a whole fleet of per-instance systems in one call.
+* ``LinearStateEstimator`` (kalman.py:109-152) for a batch of B estimators that share (A, B, C, D, L) or carry one system per
+  instance: ``predict(u)`` does ``x <- A x + B u; y <- C x`` (kalman.py:126-129) and ``update(y_meas)`` does
+  ``x <- x + L (y_meas - y)`` (kalman.py:131-133, ``y`` is not refreshed — as in the reference).  The state stays on the device;
+  ``device_state()`` feeds ``MPCController.update_from_device``.
+
+Batching follows ``MPCController``: a 2-D array is shared by every instance, a 3-D array carries a leading batch dimension.
 """
 import ctypes
 
@@ -15,19 +20,137 @@ from . import _lib
 from ._lib import BmpcError, ptr
 
 
+_DARE_STATUS = {-1: "no stabilising solution", -2: "R not positive definite"}
+_T = lambda a: np.swapaxes(a, -1, -2)
+
+
+def _arrays(names, arrays):
+    """float arrays of 2 or 3 dimensions and the common leading batch size of the 3-D ones (None when all are 2-D)"""
+    out, sizes = [], set()
+    for name, a in zip(names, arrays):
+        a = np.asarray(a, float)
+        if a.ndim not in (2, 3):
+            raise ValueError(f"{name} should be a matrix (2-D) or a batch of matrices (3-D), got shape {a.shape}")
+        if a.ndim == 3:
+            sizes.add(a.shape[0])
+        out.append(a)
+    if len(sizes) > 1:
+        raise ValueError(f"batched arrays disagree on the batch size: {sorted(sizes)}")
+    return out, (sizes.pop() if sizes else None)
+
+
+def dare(A, B, Q, R, S=None, E=None, return_status=False, device=0):
+    """Stabilising solution of the discrete algebraic Riccati equation, python-control's ``dare(A, B, Q, R, S, E)`` with E = I:
+
+        X = A'XA - (A'XB + S)(R + B'XB)^-1 (B'XA + S') + Q,      G = (R + B'XB)^-1 (B'XA + S')
+
+    Returns ``(X, L, G)`` in python-control's order, L the closed-loop eigenvalues eig(A - B G).  Any argument may carry a
+    leading batch dimension (one system per instance); all instances are solved in one call on the GPU (1 <= n, m <= 32).
+    An instance without a stabilising solution, or with R not positive definite, raises ``numpy.linalg.LinAlgError``;
+    with ``return_status=True`` the per-instance status (1 solved, -1 no stabilising solution, -2 R not positive definite)
+    is returned as a fourth element instead, and the failed instances hold NaN in X, G and L."""
+    names = ("A", "B", "Q", "R") + (() if S is None else ("S",))
+    arrs, batch = _arrays(names, (A, B, Q, R) + (() if S is None else (S,)))
+    A, B, Q, R = arrs[:4]; S = arrs[4] if S is not None else None
+    n, m = A.shape[-1], B.shape[-1]
+    want = {"A": (n, n), "B": (n, m), "Q": (n, n), "R": (m, m), "S": (n, m)}
+    for name, a in zip(names, arrs):
+        if a.shape[-2:] != want[name]:
+            raise ValueError(f"{name} should have shape {want[name]} (n = {n} states, m = {m} inputs), got {a.shape[-2:]}")
+    if not (1 <= n <= 32 and 1 <= m <= 32):
+        raise ValueError(f"dare supports 1 <= n, m <= 32 (got n = {n}, m = {m})")
+    if E is not None:
+        E = np.asarray(E, float)
+        if E.shape[-2:] != (n, n) or not np.array_equal(E, np.broadcast_to(np.eye(n), E.shape)):
+            raise ValueError("dare: only E = I (or None) is supported")
+    nb = 1 if batch is None else batch
+    full = lambda a: np.ascontiguousarray(np.broadcast_to(a, (nb,) + a.shape[-2:]))
+    A, B, Q, R = full(A), full(B), full(Q), full(R)
+    S = None if S is None else full(S)
+    L = _lib.load()
+    X = np.empty((nb, n, n)); G = np.empty((nb, m, n)); st = np.empty(nb, np.int32); it = np.empty(nb, np.int32)
+    rc = L.bmpc_dare(n, m, nb, int(device), ptr(A), ptr(B), ptr(Q), ptr(R), ptr(S), ptr(X), ptr(G), ptr(st), ptr(it))
+    if rc < 0:
+        raise BmpcError(f"bmpc_dare failed ({rc}): {L.bmpc_last_error(None).decode()}")
+    ok = st == 1
+    W = np.full((nb, n), np.nan, complex)
+    if ok.any():
+        W[ok] = np.linalg.eigvals(A[ok] - B[ok] @ G[ok])
+    if not ok.all() and not return_status:
+        bad = np.flatnonzero(~ok)[:8]
+        raise np.linalg.LinAlgError("dare: " + ", ".join(f"instance {b}: {_DARE_STATUS.get(int(st[b]), st[b])} (status {st[b]})"
+                                                         for b in bad) + (" ..." if (~ok).sum() > len(bad) else ""))
+    out = (X, W, G) if batch is not None else (X[0], W[0], G[0])
+    return out + ((st if batch is not None else st[:1]),) if return_status else out
+
+
+def kalman_design(A, B, C, D, Qn, Rn, Nn=None, return_status=False, device=0):
+    """General Kalman design (kalman.py:24-70) for x+ = A x + B [u; w], y = C x + D [u; w] + v with E[ww'] = Qn, E[vv'] = Rn,
+    E[wv'] = Nn: the last nw = Qn.shape[0] columns of B and D carry the noise w.  Returns ``(L, P, W)``: gain, Riccati
+    solution and closed-loop eigenvalues.  Batched like ``dare``."""
+    (A, B, C, D, Qn, Rn), _ = _arrays(("A", "B", "C", "D", "Qn", "Rn"), (A, B, C, D, Qn, Rn))
+    nw = Qn.shape[-1]; nu = B.shape[-1] - nw; ny = C.shape[-2]
+    if nu < 0 or D.shape[-1] != B.shape[-1] or D.shape[-2] != ny or Rn.shape[-2:] != (ny, ny):
+        raise ValueError("kalman_design: B [nx, nu + nw] and D [ny, nu + nw] must hold the nw = Qn.shape[0] noise inputs last, "
+                         "and Rn must be [ny, ny]")
+    Nn = np.zeros((nw, ny)) if Nn is None else _arrays(("Nn",), (Nn,))[0][0]
+    Bw, Dw = B[..., nu:], D[..., nu:]
+    Hn = Dw @ Nn                                                   # kalman.py:58
+    Rb = Rn + Hn + _T(Hn) + Dw @ Qn @ _T(Dw)                       # kalman.py:59
+    Qb = Bw @ Qn @ _T(Bw)                                          # kalman.py:60
+    Nb = Bw @ (Qn @ _T(Dw) + Nn)                                   # kalman.py:61
+    Qb = (Qb + _T(Qb)) / 2; Rb = (Rb + _T(Rb)) / 2                 # kalman.py:64-65
+    res = dare(_T(A), _T(C), Qb, Rb, Nb, return_status=return_status, device=device)      # kalman.py:67
+    P, W, K = res[:3]
+    return (_T(K), P, W) + tuple(res[3:])                          # kalman.py:69-70
+
+
+def kalman_design_simple(A, B, C, D, Qn, Rn, type='filter', return_status=False, device=0):
+    """Simplified Kalman design (kalman.py:73-106) for x+ = A x + B u + w, y = C x + D u + v with E[ww'] = Qn, E[vv'] = Rn:
+    ``type='filter'`` gives L = P C' (C P C' + Rn)^-1, ``'predictor'`` L = A P C' (C P C' + Rn)^-1.  Returns ``(L, P, W)``.
+    B and D are not used (as in the reference).  Batched like ``dare``."""
+    if type not in ('filter', 'predictor'):
+        raise ValueError("Unknown Kalman design type. Specify either filter or predictor!")
+    (A, C, Qn, Rn), _ = _arrays(("A", "C", "Qn", "Rn"), (A, C, Qn, Rn))
+    res = dare(_T(A), _T(C), Qn, Rn, return_status=return_status, device=device)          # kalman.py:96
+    P, W = res[0], res[1]
+    with np.errstate(invalid="ignore"):
+        PCt = P @ _T(C)
+        Sinv = np.linalg.inv(C @ PCt + Rn)
+        L = PCt @ Sinv if type == 'filter' else A @ PCt @ Sinv                           # kalman.py:99-102
+    return (L, P, W) + tuple(res[3:])
+
+
 class LinearStateEstimator:
     def __init__(self, x0, A, B, C, D, L, batch=None, device=0):
+        """Any of A, B, C, L may carry a leading batch dimension (one system per instance); `batch` then defaults to it."""
         self._L = _lib.load()
-        A = np.ascontiguousarray(A, float); B = np.ascontiguousarray(B, float).reshape(A.shape[0], -1)
-        C = np.ascontiguousarray(C, float).reshape(-1, A.shape[0]); Lg = np.ascontiguousarray(L, float).reshape(A.shape[0], -1)
+        self._per = any(np.ndim(a) == 3 for a in (A, B, C, L))
+        if not self._per:
+            A = np.ascontiguousarray(A, float); B = np.ascontiguousarray(B, float).reshape(A.shape[0], -1)
+            C = np.ascontiguousarray(C, float).reshape(-1, A.shape[0]); Lg = np.ascontiguousarray(L, float).reshape(A.shape[0], -1)
+        else:
+            (A, B, C, Lg), nb = _arrays(("A", "B", "C", "L"), (A, B, C, L))
+            if batch is None:
+                batch = nb
+            elif int(batch) != nb:
+                raise ValueError(f"batch = {batch} but the per-instance matrices carry {nb} systems")
+            full = lambda a: np.ascontiguousarray(np.broadcast_to(a, (nb,) + a.shape[-2:]))
+            A, B, C, Lg = full(A), full(B), full(C), full(Lg)
         self.A, self.B, self.C, self.D, self.L = A, B, C, np.asarray(D, float), Lg
-        self.nx, self.nu, self.ny = A.shape[0], B.shape[1], C.shape[0]
+        self.nx, self.nu, self.ny = A.shape[-1], B.shape[-1], C.shape[-2]
+        if B.shape[-2] != self.nx or C.shape[-1] != self.nx or Lg.shape[-2:] != (self.nx, self.ny):
+            raise ValueError("LinearStateEstimator: A [nx, nx], B [nx, nu], C [ny, nx] and L [nx, ny] do not agree")
         self.batch = batch
         self._B = 1 if batch is None else int(batch)
         x0 = np.ascontiguousarray(np.broadcast_to(np.asarray(x0, float).reshape(-1, self.nx), (self._B, self.nx)))
         h = ctypes.c_void_p()
-        rc = self._L.bmpc_est_create(self.nx, self.nu, self.ny, self._B, int(device), ptr(A), ptr(B), ptr(C), ptr(Lg), ptr(x0),
-                                     ctypes.byref(h))
+        if not self._per:
+            rc = self._L.bmpc_est_create(self.nx, self.nu, self.ny, self._B, int(device), ptr(A), ptr(B), ptr(C), ptr(Lg), ptr(x0),
+                                         ctypes.byref(h))
+        else:
+            rc = self._L.bmpc_est_create_ex(self.nx, self.nu, self.ny, self._B, self._B, int(device), ptr(A), ptr(B), ptr(C),
+                                            ptr(Lg), ptr(x0), ctypes.byref(h))
         if rc < 0:
             raise BmpcError(f"bmpc_est_create failed ({rc}): {self._L.bmpc_last_error(None).decode()}")
         self._h = h
@@ -83,6 +206,8 @@ class LinearStateEstimator:
 
     def sim(self, u_seq, x=None):
         """Open-loop output prediction on the host, as the reference does (kalman.py:136-152); B = 1 only."""
+        if self._per:
+            raise ValueError("sim() predicts one instance of a shared system; this estimator has one system per instance")
         x = np.array(self.x if x is None else x, float).reshape(-1)
         u_seq = np.asarray(u_seq, float).reshape(len(u_seq), -1)
         assert u_seq.shape[1] == self.nu
