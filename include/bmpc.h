@@ -81,6 +81,7 @@ typedef struct {
     float ms_polish;            /* device time of the polish kernels */
     int32_t launches;           /* kernels launched by the last solve */
     int32_t infeasible;         /* instances certified primal infeasible (status -3) in the last solve */
+    int32_t recondensed;        /* per-instance systems: condensed blocks the last solve brought up to date after bmpc_update_system */
 } bmpc_stats;
 
 void bmpc_default_config(bmpc_config* cfg);
@@ -103,6 +104,19 @@ int bmpc_setup(bmpc_handle* h, const double* Ad, const double* Bd, const double*
  * on_device = 2: device pointers that are BORROWED — the solver kernels read x0 / uminus1 in place, no copy; the caller leaves
  * them unchanged until the next solve has been retired (bmpc_output, bmpc_synchronize); xref is always copied. */
 int bmpc_update(bmpc_handle* h, const double* x0, const double* uminus1, const double* xref, int xref_rows, int on_device);
+
+/* time-varying system matrices (doc/latex/main.tex:505-511: with time-varying Ad and Bd the prediction matrices have to be
+ * updated at every MPC iteration): replace (Ad, Bd) of every system of an already set-up handle; weights, bounds, uref and rho are unchanged.
+ * Ad [n_sys,nx,nx], Bd [n_sys,nx,nu], row-major, batch-major; either may be NULL (keep).  on_device = 0: host pointers, 1: device
+ * pointers on this handle's device (stream-ordered; the caller keeps them unchanged until the next solve has been retired).
+ * A pending solve is retired first.  The warm-start state — working sets, v*, the per-instance rho level, the committed u_-1, the
+ * cold/warm flag — is kept: the next bmpc_solve is a WARM solve of the QP the reference would assemble with the new matrices.
+ * rho keeps the value the setup chose (the exact answer does not depend on it).
+ * n_sys = 1: the system is condensed again at once and checked like bmpc_setup.  n_sys = batch: when P_X >= 0 and P_U > 0 (decided
+ * at setup) H is positive definite for any (Ad, Bd) and each instance is condensed again only before the first launch that reads its
+ * condensed block — a warm solve that the fast-path polish finishes alone condenses nothing; otherwise all instances at once.
+ * BMPC_ERR_NOT_PD: bmpc_solve returns BMPC_ERR_STATE until a successful bmpc_update_system or bmpc_setup. */
+int bmpc_update_system(bmpc_handle* h, const double* Ad, const double* Bd, int on_device);
 
 /* replaces OSQP.solve (mpc.py:366-375): K3 + K4 + K5 */
 int bmpc_solve(bmpc_handle* h);

@@ -28,9 +28,11 @@
 // unpolished" on tight ADMM residuals.
 // [10..11] / [12..13]: ~(earliest start) and latest end of k_tpi_pol in ns of the GPU's global timer (64-bit each): the kernel's
 // own duration, for the roofline of bench.py (CUDA events around a launch also count launch gaps).
+// [9]: instances re-condensed by k_condense_list in this round (rounds that report through a D2H copy; in the mapped-memory report of
+// k_tpi_pol slot 9 carries the K6 arrival flag instead — those rounds never condense).
 // [14]: warps of k_tpi_pol that have left; the last one copies the block into the handle's MAPPED pinned host buffer and raises
 // [15] = launch epoch there: the host spins on that word instead of paying a D2H copy + stream synchronisation per solve.
-enum { TPI_Q_CURSOR = 4, TPI_Q_HEAD = 5, TPI_Q_TAIL = 6, BMPC_CNT_TIGHT = 8, BMPC_CNT_T0 = 10, BMPC_CNT_T1 = 12, BMPC_CNT_EXIT = 14, BMPC_CNT_EPOCH = 15, BMPC_CNT = 16 };
+enum { TPI_Q_CURSOR = 4, TPI_Q_HEAD = 5, TPI_Q_TAIL = 6, BMPC_CNT_TIGHT = 8, BMPC_CNT_COND = 9, BMPC_CNT_T0 = 10, BMPC_CNT_T1 = 12, BMPC_CNT_EXIT = 14, BMPC_CNT_EPOCH = 15, BMPC_CNT = 16 };
 __device__ __forceinline__ unsigned long long bmpc_globaltimer() { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); return t; }
 
 // ------------------------------------------------------------------------------------------------
@@ -176,6 +178,53 @@ __global__ void k_condense(BmpcDims d, BmpcSysOff o, double* sys, double rho, do
     __shared__ int si[32];
     BlockTeam t(sd, si);
     bmpc_condense(t, d, o, sys + (size_t)blockIdx.x * o.total, rho, sigma, alpha, eps_feas, soft_on);
+}
+
+// ---- time-varying (Ad, Bd) without a new setup (bmpc_update_system)
+// k_sys_refresh: one thread per (field, instance), field-major so that the stores into the fast path's field-major parameter view
+// (TpiPolView: field f of instance i at view[f * B + i]) are coalesced.  Writes the new Ad / Bd (batch-major, row-major; either may
+// be null) into every instance's system block and, when the handle has one, into the view's Ad / Bd fields (view_ad / view_bd: field
+// numbers).  The condensed part of the block is NOT touched here: the handle's generation counter has moved past every instance's
+// stamp, and k_condense_list re-condenses an instance before the first launch that reads its condensed block.
+__global__ void k_sys_refresh(BmpcDims d, BmpcSysOff o, double* __restrict__ sys, size_t sys_stride, int B, const double* __restrict__ Ad,
+                              const double* __restrict__ Bd, double* __restrict__ view, int view_ad, int view_bd) {
+    const int nA = Ad ? d.nx * d.nx : 0, nB = Bd ? d.nx * d.nu : 0;
+    const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= (size_t)B * (nA + nB)) return;
+    const int f = (int)(idx / B), inst = (int)(idx % B);
+    double* blk = sys + (size_t)inst * sys_stride;
+    if (f < nA) {
+        const double v = Ad[(size_t)inst * nA + f];
+        blk[o.Ad + f] = v;
+        if (view) view[(size_t)(view_ad + f) * B + inst] = v;
+    } else {
+        const int e = f - nA;
+        const double v = Bd[(size_t)inst * nB + e];
+        blk[o.Bd + e] = v;
+        if (view) view[(size_t)(view_bd + e) * B + inst] = v;
+    }
+}
+
+// k_condense_list: K1 over the listed instances (list == nullptr: 0..count-1), one CTA each, with the rho the setup chose (read from
+// the instance's own block: the ladder, the per-instance level and the staged v* = z* + y*/rho stay consistent).  gen != nullptr:
+// instances whose stamp already equals `cur` are fresh and leave at once; the others are condensed and stamped.  ncount: number of
+// instances condensed (per-solve statistics), may be null.
+__global__ void k_condense_list(BmpcDims d, BmpcSysOff o, double* sys, size_t sys_stride, const int32_t* __restrict__ list, int count,
+                                int32_t* gen, int32_t cur, double sigma, double alpha, double eps_feas, int soft_on, int32_t* ncount) {
+    __shared__ double sd[32];
+    __shared__ int si[32];
+    const int idx = blockIdx.x;
+    if (idx >= count) return;
+    const int inst = list ? list[idx] : idx;
+    if (gen && gen[inst] == cur) return;
+    double* blk = sys + (size_t)inst * sys_stride;
+    const double rho = blk[o.scal + BMPC_S_RHO];           // read before the condense rewrites scal (behind its first barrier)
+    BlockTeam t(sd, si);
+    bmpc_condense(t, d, o, blk, rho, sigma, alpha, eps_feas, soft_on);
+    if (t.tid == 0) {
+        if (gen) gen[inst] = cur;
+        if (ncount) atomicAdd(ncount, 1);
+    }
 }
 
 template <bool WARP>
@@ -991,6 +1040,7 @@ struct TpiEntry {
     size_t admm_bytes, ric_bytes; int code_stride;
     void (*fill)(const double* hs, const BmpcSysOff& o, void* pa, void* pp);
     int view_fields; void (*fill_view)(struct bmpc_handle* h);
+    int view_ad, view_bd;              // field numbers of Ad and Bd in the per-instance parameter view (k_sys_refresh)
     int (*configure)();
     void (*launch)(struct bmpc_handle* h, const int32_t* list, int count, int niter, int32_t* next_list, cudaEvent_t mid);
     void (*launch_polish)(struct bmpc_handle* h, const int32_t* list, int count, int32_t* next_list);
@@ -1043,6 +1093,7 @@ struct bmpc_handle {
     int tpm_kind = 0;                  // 0 none, else 1 + index into g_tpm_table (compiled multi-input fast-path shapes)
     void* tpm_params = nullptr;        // host copy of the parameter block
     double* tpm_W = nullptr; unsigned long long* tpm_rec = nullptr;   // gain rows of the resident warps, working-set records
+    int tpm_W_slots = 0;               // gain slots per lane tpm_W was allocated for
     // refinements of the first launch / of a straggler round, ADMM iterations of the first straggler round.  (12, 4, 100) was measured on
     // the MIMO side bench with the all-at-once update in the straggler rounds too (tools/sweep_tpm_caps.sh: 13.3 ms/step at 8,6,25 ->
     // 11.4 ms); the straggler rounds now run in exchange mode, where 12 refinements finish every straggler of the host study in the
@@ -1052,6 +1103,14 @@ struct bmpc_handle {
     // first polish after 25 iterations: cap 4 verifies none and the solve takes 333 iterations in 4.5 rounds, cap 12 79 %, cap 16 92 %,
     // cap 24 all of them in the first round; after 50 iterations the same picture): every polish attempt of a cold solve gets this cap
     int tpm_cold_cap = 24;
+    // time-varying (Ad, Bd), bmpc_update_system.  Per-instance systems: every instance's condensed block carries the generation it
+    // was condensed for (sys_gen[i]); bmpc_update_system moves the handle's counter ahead of all of them and k_condense_list brings
+    // an instance up to date right before the first launch that reads its condensed block.
+    int32_t* sys_gen = nullptr; int32_t sys_gen_cur = 0;
+    bool sys_stale = false;            // some instance's condensed block may predate its (Ad, Bd)
+    bool sys_lazy = false;             // H is positive definite whatever (Ad, Bd) are (decided at setup): the condense may be deferred
+    bool sys_bad = false;              // the last bmpc_update_system failed the positive-definiteness check: bmpc_solve refuses
+    double* sys_stage = nullptr;       // device copy of host (Ad, Bd) for k_sys_refresh
 };
 
 static std::string g_create_err;
@@ -1138,6 +1197,10 @@ static void tpi_fill_view_entry(bmpc_handle* h) {
     k_tpi_fill_view<S><<<(B + 63) / 64, 64, 0, h->stream>>>(h->o, h->sys, (size_t)h->o.total, B, h->tpi_view);
 }
 template <class S>
+static constexpr int tpi_view_field_ad() { using PS = TpiPolParams<S>; return (int)(offsetof(PS, Ad) / sizeof(double)); }
+template <class S>
+static constexpr int tpi_view_field_bd() { using PS = TpiPolParams<S>; return (int)(offsetof(PS, Bd) / sizeof(double)); }
+template <class S>
 static int tpi_configure_entry() {
     if (cudaFuncSetAttribute(k_tpi_admm<S, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(S::MT * TPI_STR * 8)) != cudaSuccess) return 1;
     if (cudaFuncSetAttribute(k_tpi_admm<S, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(S::MT * TPI_STR * 8)) != cudaSuccess) return 1;
@@ -1152,6 +1215,7 @@ static int tpi_configure_entry() {
     {NX_, NU_, NP_, NC_, sizeof(TpiAdmmParams<TpiShape<NX_, NU_, NP_, NC_>>), sizeof(TpiPolParams<TpiShape<NX_, NU_, NP_, NC_>>), \
      TpiPolLayout<TpiShape<NX_, NU_, NP_, NC_>>::code_stride,                                                                \
      tpi_fill_entry<TpiShape<NX_, NU_, NP_, NC_>>, TpiPolView<TpiShape<NX_, NU_, NP_, NC_>>::NF, tpi_fill_view_entry<TpiShape<NX_, NU_, NP_, NC_>>, \
+     tpi_view_field_ad<TpiShape<NX_, NU_, NP_, NC_>>(), tpi_view_field_bd<TpiShape<NX_, NU_, NP_, NC_>>(),                   \
      tpi_configure_entry<TpiShape<NX_, NU_, NP_, NC_>>,                                                                        \
      launch_tpi_round<TpiShape<NX_, NU_, NP_, NC_>>, launch_tpi_polish_only<TpiShape<NX_, NU_, NP_, NC_>>},
 // BMPC_TPI_SHAPES_FILE: pympc_b200.build.jit_shape() compiles a copy of the library whose table holds the one shape a controller
@@ -1402,6 +1466,8 @@ void bmpc_destroy(bmpc_handle* h) {
     if (h->tpi_view) cudaFree(h->tpi_view);
     if (h->tpm_W) cudaFree(h->tpm_W);
     if (h->tpm_rec) cudaFree(h->tpm_rec);
+    if (h->sys_gen) cudaFree(h->sys_gen);
+    if (h->sys_stage) cudaFree(h->sys_stage);
     for (int i = 0; i < 4; i++) if (h->ev[i]) cudaEventDestroy(h->ev[i]);
     if (h->own_stream) cudaStreamDestroy(h->own_stream);
     delete h;
@@ -1467,6 +1533,77 @@ int bmpc_get_dims(const bmpc_handle* h, int32_t* dims) {
     return BMPC_OK;
 }
 
+// ---- helpers of bmpc_setup and bmpc_update_system
+// x'Qx > 0 for every x != 0: Cholesky factorisation of the symmetric part
+static bool host_pd(const double* Q, int n) {
+    std::vector<double> L((size_t)n * n);
+    for (int i = 0; i < n; i++) for (int j = 0; j < n; j++) L[i * n + j] = 0.5 * (Q[i * n + j] + Q[j * n + i]);
+    for (int j = 0; j < n; j++) {
+        double s = L[j * n + j];
+        for (int k = 0; k < j; k++) s -= L[j * n + k] * L[j * n + k];
+        if (!(s > 0.0)) return false;
+        L[j * n + j] = sqrt(s);
+        for (int i = j + 1; i < n; i++) {
+            double t = L[i * n + j];
+            for (int k = 0; k < j; k++) t -= L[i * n + k] * L[j * n + k];
+            L[i * n + j] = t / L[j * n + j];
+        }
+    }
+    return true;
+}
+// x'Qx >= 0 for every x: a diagonal with non-negative entries, or positive definite (a singular non-diagonal Q counts as "no")
+static bool host_psd(const double* Q, int n) {
+    bool diag = true, nonneg = true;
+    for (int i = 0; i < n; i++) for (int j = 0; j < n; j++) {
+        if (i != j && Q[i * n + j] != 0.0) diag = false;
+        if (i == j && !(Q[i * n + j] >= 0.0)) nonneg = false;
+    }
+    return diag ? nonneg : host_pd(Q, n);
+}
+
+// multi-input fast path: the first compiled entry of the shape whose (Ad, Bd) pattern masks contain the system's (blk: system block
+// on the host, inputs at their block offsets); 0: none
+static bool tpm_eligible(const bmpc_handle* h) {
+    return h->cfg.fast_path && !h->tpi_kind && h->cfg.soft_on && h->cfg.n_sys <= 1 && h->cfg.polish;
+}
+static int tpm_match(const bmpc_handle* h, const double* blk) {
+    const BmpcDims& d = h->d; const BmpcSysOff& o = h->o;
+    unsigned long long am = 0ull; unsigned bm = 0u;
+    if (d.nx * d.nx <= 64 && d.nx * d.nu <= 32) {
+        for (int i = 0; i < d.nx * d.nx; i++) if (blk[o.Ad + i] != 0.0) am |= 1ull << i;
+        for (int i = 0; i < d.nx * d.nu; i++) if (blk[o.Bd + i] != 0.0) bm |= 1u << i;
+    } else { am = ~0ull; bm = ~0u; }
+    for (int k = 0; k < g_tpm_count; k++)
+        if (g_tpm_table[k].nx == d.nx && g_tpm_table[k].nu == d.nu && g_tpm_table[k].Np == d.Np && g_tpm_table[k].Nc == d.Nc &&
+            (am & ~g_tpm_table[k].amask) == 0ull && (bm & ~g_tpm_table[k].bmask) == 0u) return k + 1;
+    return 0;
+}
+// parameter block and workspace of multi-input entry `kind` from the condensed block hs (host copy); the entry stays off when its
+// fill declines (QDu not diagonal: team kernels).  fresh: the stored working-set records start empty (the next warm solve reads
+// its working sets off v*)
+static int tpm_prepare(bmpc_handle* h, const double* hs, int kind, bool fresh) {
+    const TpmEntry& te = g_tpm_table[kind - 1];
+    free(h->tpm_params); h->tpm_params = malloc(te.par_bytes);
+    h->tpm_kind = te.fill(hs, h->o, h->tpm_params) ? kind : 0;
+    if (!h->tpm_kind) return BMPC_OK;
+    const size_t B = h->cfg.batch, nwarp = (B + 31) / 32;
+    if (h->tpm_W && h->tpm_W_slots < te.slots) { cudaFree(h->tpm_W); h->tpm_W = nullptr; }
+    if (!h->tpm_W) { BMPC_CUDA(cudaMalloc((void**)&h->tpm_W, sizeof(double) * nwarp * 32 * (size_t)te.slots)); h->tpm_W_slots = te.slots; }
+    if (!h->tpm_rec) { BMPC_CUDA(cudaMalloc((void**)&h->tpm_rec, sizeof(unsigned long long) * B * (size_t)(h->d.Np + 2))); fresh = true; }
+    if (fresh) BMPC_CUDA(cudaMemsetAsync(h->tpm_rec, 0, sizeof(unsigned long long) * B * (size_t)(h->d.Np + 2), h->stream));
+    return BMPC_OK;
+}
+
+// per-instance systems after bmpc_update_system: bring the condensed blocks of the listed instances (nullptr: 0..count-1) up to date
+// before a launch that reads them; instances already fresh cost one CTA that leaves at once.  Returns 1 if it launched.
+static int condense_stale(bmpc_handle* h, const int32_t* list, int count, int32_t* ncount) {
+    if (!h->sys_stale || count <= 0) return 0;
+    k_condense_list<<<count, 256, 0, h->stream>>>(h->d, h->o, h->sys, h->I.sys_stride, list, count, h->sys_gen, h->sys_gen_cur,
+                                                  h->cfg.sigma, h->cfg.alpha, h->cfg.eps_feas, h->cfg.soft_on, ncount);
+    if (list == nullptr && count >= h->cfg.batch) h->sys_stale = false;
+    return 1;
+}
+
 int bmpc_setup(bmpc_handle* h, const double* Ad, const double* Bd, const double* Qx, const double* QxN, const double* Qu,
                const double* QDu, const double* xmin, const double* xmax, const double* umin, const double* umax,
                const double* Dumin, const double* Dumax, const double* uref) {
@@ -1522,34 +1659,34 @@ int bmpc_setup(bmpc_handle* h, const double* Ad, const double* Bd, const double*
         }
     }
     // multi-input fast path: compiled shape, one shared system, soft state rows, diagonal QDu
+    // (sparsity pattern of (Ad, Bd): an entry fits when its compile-time masks contain it)
     h->tpm_kind = 0;
-    if (h->cfg.fast_path && !h->tpi_kind && h->cfg.soft_on && ns == 1 && h->cfg.polish) {
-        // sparsity pattern of (Ad, Bd): an entry fits when its compile-time masks contain it
-        unsigned long long am = 0ull; unsigned bm = 0u;
-        if (d.nx * d.nx <= 64 && d.nx * d.nu <= 32) {
-            for (int i = 0; i < d.nx * d.nx; i++) if (in[o.Ad + i] != 0.0) am |= 1ull << i;
-            for (int i = 0; i < d.nx * d.nu; i++) if (in[o.Bd + i] != 0.0) bm |= 1u << i;
-        } else { am = ~0ull; bm = ~0u; }
-        for (int k = 0; k < g_tpm_count; k++)
-            if (g_tpm_table[k].nx == d.nx && g_tpm_table[k].nu == d.nu && g_tpm_table[k].Np == d.Np && g_tpm_table[k].Nc == d.Nc &&
-                (am & ~g_tpm_table[k].amask) == 0ull && (bm & ~g_tpm_table[k].bmask) == 0u) { h->tpm_kind = k + 1; break; }
-    }
-    if (h->tpm_kind) {
-        const TpmEntry& te = g_tpm_table[h->tpm_kind - 1];
+    const int tk = tpm_eligible(h) ? tpm_match(h, in.data()) : 0;
+    if (tk) {
         std::vector<double> hs(o.total);
         BMPC_CUDA(cudaMemcpyAsync(hs.data(), h->sys, sizeof(double) * o.total, cudaMemcpyDeviceToHost, h->stream));
         BMPC_CUDA(cudaStreamSynchronize(h->stream));
-        free(h->tpm_params); h->tpm_params = malloc(te.par_bytes);
-        if (!te.fill(hs.data(), o, h->tpm_params)) h->tpm_kind = 0;      // QDu not diagonal: team kernels
+        int rc = tpm_prepare(h, hs.data(), tk, true);
+        if (rc) return rc;
     }
     if (h->tpm_kind) {
         if (const char* e = getenv("BMPC_TPM_CAPS")) sscanf(e, "%d,%d,%d,%d", &h->tpm_first_cap, &h->tpm_round_cap, &h->tpm_chunk, &h->tpm_cold_cap);   // tuning knob (tools/gpu_sweep.py)
-        const TpmEntry& te = g_tpm_table[h->tpm_kind - 1];
-        const size_t B = h->cfg.batch, nwarp = (B + 31) / 32;
-        if (!h->tpm_W) BMPC_CUDA(cudaMalloc((void**)&h->tpm_W, sizeof(double) * nwarp * 32 * (size_t)te.slots));
-        if (!h->tpm_rec) BMPC_CUDA(cudaMalloc((void**)&h->tpm_rec, sizeof(unsigned long long) * B * (size_t)(d.Np + 2)));
-        BMPC_CUDA(cudaMemsetAsync(h->tpm_rec, 0, sizeof(unsigned long long) * B * (size_t)(d.Np + 2), h->stream));
     }
+    // time-varying (Ad, Bd) on per-instance systems: H = B'P_X B + P_U is positive definite for ANY (Ad, Bd) when P_X >= 0 and
+    // P_U > 0 (Qu, QDu >= 0 and one of them > 0: the difference matrix T is positive definite) — then bmpc_update_system may defer
+    // the condense to the launches that need it
+    h->sys_lazy = false;
+    if (ns > 1) {
+        h->sys_lazy = true;
+        for (int si = 0; si < ns && h->sys_lazy; si++) {
+            const double* blk = in.data() + (size_t)si * o.pw;
+            h->sys_lazy = host_psd(blk + o.Qx, d.nx) && host_psd(blk + o.QxN, d.nx) && host_psd(blk + o.Qu, d.nu) && host_psd(blk + o.QDu, d.nu) &&
+                          (host_pd(blk + o.Qu, d.nu) || host_pd(blk + o.QDu, d.nu));
+        }
+        if (!h->sys_gen) BMPC_CUDA(cudaMalloc((void**)&h->sys_gen, sizeof(int32_t) * (size_t)ns));
+        BMPC_CUDA(cudaMemsetAsync(h->sys_gen, 0, sizeof(int32_t) * (size_t)ns, h->stream));
+    }
+    h->sys_gen_cur = 0; h->sys_stale = false; h->sys_bad = false;
     // uminus1 default = uref for every instance (mpc.py:141); caller overrides through bmpc_update
     h->is_setup = true; h->cold = true; h->solved = false; h->pending = false; h->codes_valid = false;
     return BMPC_OK;
@@ -1579,6 +1716,79 @@ int bmpc_update(bmpc_handle* h, const double* x0, const double* uminus1, const d
         h->xref_mode = xref_rows == 1 ? 0 : 1;
         BMPC_CUDA(cudaMemcpyAsync(h->xref, xref, sizeof(double) * B * (h->xref_mode ? d.NX : d.nx), kind, h->stream));
     }
+    return BMPC_OK;
+}
+
+// condensed Hessians of all n_sys systems positive definite (the check of bmpc_setup); otherwise solves are refused until the next
+// successful bmpc_update_system / bmpc_setup
+static int check_condensed(bmpc_handle* h) {
+    const int ns = h->cfg.n_sys; const BmpcSysOff& o = h->o;
+    std::vector<double> errs(ns);
+    BMPC_CUDA(cudaMemcpy2DAsync(errs.data(), sizeof(double), h->sys + o.scal + BMPC_S_ERR, sizeof(double) * o.total, sizeof(double), ns,
+                                cudaMemcpyDeviceToHost, h->stream));
+    BMPC_CUDA(cudaStreamSynchronize(h->stream));
+    for (int si = 0; si < ns; si++) if (errs[si] != 0.0) {
+        h->sys_bad = true;
+        h->err = "bmpc_update_system: condensed Hessian is not positive definite (Qu/QDu/Qx with the new (Ad, Bd) make the QP non-strictly convex in U)";
+        return BMPC_ERR_NOT_PD;
+    }
+    return BMPC_OK;
+}
+
+int bmpc_update_system(bmpc_handle* h, const double* Ad, const double* Bd, int on_device) {
+    if (!h) return BMPC_ERR_ARG;
+    if (!h->is_setup) { h->err = "bmpc_update_system before bmpc_setup"; return BMPC_ERR_STATE; }
+    if (on_device != 0 && on_device != 1) { h->err = "bmpc_update_system: on_device must be 0 (host) or 1 (device)"; return BMPC_ERR_ARG; }
+    BMPC_CUDA(cudaSetDevice(h->cfg.device));
+    if (h->pending) { int rc = finish_solve(h); if (rc) return rc; }
+    if (!Ad && !Bd) return BMPC_OK;
+    const BmpcDims& d = h->d; const BmpcSysOff& o = h->o;
+    const size_t nA = (size_t)d.nx * d.nx, nB = (size_t)d.nx * d.nu;
+    if (h->cfg.n_sys <= 1) {
+        // shared system: eager.  New inputs into the block, K1 with the kept rho, the check of bmpc_setup, then everything that was
+        // derived from the condensed block on the host: the fast paths' constant-bank parameters and the choice of the multi-input entry
+        // (a pattern that leaves the compiled masks must not be answered by a kernel that skips those entries)
+        const cudaMemcpyKind kind = on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+        if (Ad) BMPC_CUDA(cudaMemcpyAsync(h->sys + o.Ad, Ad, sizeof(double) * nA, kind, h->stream));
+        if (Bd) BMPC_CUDA(cudaMemcpyAsync(h->sys + o.Bd, Bd, sizeof(double) * nB, kind, h->stream));
+        k_condense_list<<<1, 256, 0, h->stream>>>(d, o, h->sys, 0, nullptr, 1, nullptr, 0, h->cfg.sigma, h->cfg.alpha, h->cfg.eps_feas,
+                                                  h->cfg.soft_on, nullptr);
+        BMPC_CUDA(cudaGetLastError());
+        int rc = check_condensed(h);
+        if (rc) return rc;
+        std::vector<double> hs(o.total);
+        BMPC_CUDA(cudaMemcpyAsync(hs.data(), h->sys, sizeof(double) * o.total, cudaMemcpyDeviceToHost, h->stream));
+        BMPC_CUDA(cudaStreamSynchronize(h->stream));
+        if (h->tpi_kind) g_tpi_table[h->tpi_kind - 1].fill(hs.data(), o, h->tpi_admm_params, h->tpi_polish_params);
+        const int old = h->tpm_kind;
+        const int tk = tpm_eligible(h) ? tpm_match(h, hs.data()) : 0;
+        h->tpm_kind = 0;
+        if (tk) { rc = tpm_prepare(h, hs.data(), tk, tk != old); if (rc) return rc; }
+        h->sys_bad = false;
+        return BMPC_OK;
+    }
+    // per-instance systems: the new matrices go into every block and into the fast path's parameter view; the condense is deferred
+    // to the launches that read a condensed block (condense_stale) — unless H may lose definiteness, then all of it now + the check
+    const int B = h->cfg.batch;
+    const double *dA = Ad, *dB = Bd;
+    if (!on_device) {
+        if (!h->sys_stage) BMPC_CUDA(cudaMalloc((void**)&h->sys_stage, sizeof(double) * (size_t)B * (nA + nB)));
+        if (Ad) { BMPC_CUDA(cudaMemcpyAsync(h->sys_stage, Ad, sizeof(double) * B * nA, cudaMemcpyHostToDevice, h->stream)); dA = h->sys_stage; }
+        if (Bd) { BMPC_CUDA(cudaMemcpyAsync(h->sys_stage + B * nA, Bd, sizeof(double) * B * nB, cudaMemcpyHostToDevice, h->stream)); dB = h->sys_stage + B * nA; }
+    }
+    const TpiEntry* te = h->tpi_kind ? &g_tpi_table[h->tpi_kind - 1] : nullptr;
+    const size_t n = (size_t)B * ((Ad ? nA : 0) + (Bd ? nB : 0));
+    k_sys_refresh<<<(unsigned)((n + 255) / 256), 256, 0, h->stream>>>(d, o, h->sys, h->I.sys_stride, B, dA, dB, h->tpi_view,
+                                                                      te ? te->view_ad : 0, te ? te->view_bd : 0);
+    BMPC_CUDA(cudaGetLastError());
+    h->sys_gen_cur++; h->sys_stale = true;
+    if (!h->sys_lazy) {
+        condense_stale(h, nullptr, B, nullptr);
+        BMPC_CUDA(cudaGetLastError());
+        int rc = check_condensed(h);
+        if (rc) return rc;
+    }
+    h->sys_bad = false;
     return BMPC_OK;
 }
 
@@ -1655,6 +1865,9 @@ static int enqueue_round(bmpc_handle* h) {
             BMPC_CUDA(cudaMemcpyAsync(h->um1_solved, h->um1_cur, sizeof(double) * (size_t)B * h->d.nu, cudaMemcpyDefault, h->stream));   // (um1_cur may be mapped host memory)
         }
         BMPC_CUDA(cudaMemsetAsync(h->counts, 0, sizeof(int32_t) * 2 * BMPC_CNT, h->stream));     // this round's half and the next one's
+        // every launch below reads the condensed blocks of exactly this round's instances (per-instance systems after
+        // bmpc_update_system: bring them up to date first; the fast-path round above reads only the parameter view)
+        h->stats.launches += condense_stale(h, st.list, st.count, cnt + BMPC_CNT_COND);
     }
     h->spin_epoch = 0;
     if (tpi && st.chunk == 0) { h->epoch = (h->epoch % 1000000000) + 1; h->spin_epoch = h->epoch; ((volatile int32_t*)h->h_count)[BMPC_CNT_EPOCH] = 0; }
@@ -1725,6 +1938,7 @@ static int retire_round(bmpc_handle* h, int* more) {
     st.count = h->h_count[0];
     h->stats.polish_steps += h->h_count[1];
     h->stats.infeasible += h->h_count[3];
+    if (!h->spin_epoch) h->stats.recondensed += h->h_count[BMPC_CNT_COND];
     st.tight += h->h_count[BMPC_CNT_TIGHT];
     if (spun && h->h_count[BMPC_CNT_TIGHT + 1] == 1) h->g_done_epoch = h->g_epoch;
     st.list = st.nxt; int32_t* tmp = st.cur; st.cur = st.nxt; st.nxt = tmp;
@@ -1756,6 +1970,7 @@ static int finish_solve(bmpc_handle* h) {
 int bmpc_solve(bmpc_handle* h) {
     if (!h) return BMPC_ERR_ARG;
     if (!h->is_setup) { h->err = "bmpc_solve before bmpc_setup"; return BMPC_ERR_STATE; }
+    if (h->sys_bad) { h->err = "bmpc_solve after a failed bmpc_update_system (condensed Hessian not positive definite): update the system again or set up anew"; return BMPC_ERR_STATE; }
     BMPC_CUDA(cudaSetDevice(h->cfg.device));
     if (h->pending) { int rc = finish_solve(h); if (rc) return rc; }
     const int B = h->cfg.batch;
@@ -1841,6 +2056,7 @@ int bmpc_get_sequences(bmpc_handle* h, double* u_seq, double* x_seq, double* eps
         int wpb = 4;
         size_t sm = (size_t)wpb * (d.NU + d.NX + d.nu + 1) * sizeof(double);
         BMPC_CUDA(cudaFuncSetAttribute(k_sequences, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+        condense_stale(h, nullptr, (int)B, nullptr);          // k_sequences reads every instance's condensed block
         k_sequences<<<(int)((B + wpb - 1) / wpb), wpb * 32, sm, h->stream>>>(d, h->o, h->sys, h->I, (int)B, h->xref_mode, h->seq_x, h->seq_e, h->seq_obj);
         BMPC_CUDA(cudaGetLastError());
         if (x_seq) BMPC_CUDA(cudaMemcpyAsync(x_seq, h->seq_x, sizeof(double) * B * d.NX, cudaMemcpyDeviceToHost, h->stream));
@@ -1872,6 +2088,8 @@ int bmpc_get_sys(bmpc_handle* h, const char* name, double* out, int capacity) {
         {"hi0", o.hi0, d.mc}, {"rho", o.rho, d.mc}, {"scal", o.scal, BMPC_S_COUNT}};
     for (auto& e : tab) if (strcmp(e.n, name) == 0) {
         if (capacity < e.cnt) { h->err = "bmpc_get_sys: buffer too small"; return BMPC_ERR_ARG; }
+        condense_stale(h, nullptr, 1, nullptr);               // the exported block is system 0's
+        BMPC_CUDA(cudaGetLastError());
         BMPC_CUDA(cudaMemcpyAsync(out, h->sys + e.off, sizeof(double) * e.cnt, cudaMemcpyDeviceToHost, h->stream));
         BMPC_CUDA(cudaStreamSynchronize(h->stream));
         return e.cnt;

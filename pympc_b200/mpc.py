@@ -466,6 +466,66 @@ class MPCController:
         if solve:
             self.solve()
 
+    def update_system(self, Ad=None, Bd=None):
+        """Time-varying system matrices (successive linearisation, gain scheduling): replace Ad and/or Bd of the set-up controller
+        without a new setup().  The next update() is a WARM solve of the QP the reference would assemble with the new matrices
+        (working sets, ADMM state and the committed u_{-1} are kept; weights, bounds, uref and rho are unchanged).
+
+        Shared controller: 2-D Ad (nx, nx) / Bd (nx, nu).  Per-instance controller: (batch, nx, nx) / (batch, nx, nu), or 2-D to give
+        every instance the same model.  Dense arrays or scipy.sparse.  The reference-form attributes (Ad, Bd, P, A, ...) follow.
+        Assigning ``K.Ad`` directly keeps the reference's meaning: no effect until setup()."""
+        Ad, Bd = self._system_arg(Ad, "Ad", (self.nx, self.nx), "Ad should be a square matrix of dimension (nx,nx)!"), \
+            self._system_arg(Bd, "Bd", (self.nx, self.nu), "Bd should be a matrix of dimension (nx, nu)!")
+        if self._h is None:
+            raise BmpcError("update_system() before setup()")
+        if Ad is None and Bd is None:
+            return
+        B = self._B
+        full = (lambda M: None if M is None else np.ascontiguousarray(np.broadcast_to(M, (B,) + M.shape[-2:]))) if self._per_instance \
+            else (lambda M: M)
+        a, b = full(Ad), full(Bd)
+        rc = self._L.bmpc_update_system(self._h, ptr(a), ptr(b), 0)
+        # the handle holds the new matrices even when the check fails (then solve() raises until a valid update): so do the attributes
+        for name, M in (("Ad", Ad), ("Bd", Bd)):
+            if M is None:
+                continue
+            if self._per_instance:
+                self._sys_full[name] = M
+            setattr(self, name, M[0] if M.ndim == 3 else M)
+        self._qp_static = None
+        self._check(rc)
+
+    def _system_arg(self, M, name, shape, msg):
+        if M is None:
+            return None
+        M = np.array(M.toarray() if hasattr(M, "toarray") else M, dtype=float)          # a copy: the caller may reuse its buffer
+        if M.ndim == 3 and not self._per_instance:
+            raise ValueError(f"per-instance {name} of shape (batch, ...) needs a controller set up with per-instance systems "
+                             "(Ad of shape (batch, nx, nx) at construction)")
+        if M.shape not in (shape, (self._B,) + shape):
+            raise ValueError(msg)
+        return M
+
+    def update_system_from_device(self, Ad_ptr=None, Bd_ptr=None):
+        """update_system() with the matrices already on this controller's device (raw pointers, or contiguous float64 torch tensors),
+        e.g. a batch of linearisations computed by torch: no host round trip.  Layout as for update_system — per-instance
+        controllers (batch, nx, nx) / (batch, nx, nu), shared ones (nx, nx) / (nx, nu).  The library reads them in stream order on the
+        controller's stream: whatever wrote them must be ordered before (same stream, or synchronised); keep them unchanged until
+        the next solve has been retired.  The host-side attributes (Ad, Bd, P, A) keep describing the last host-side system."""
+        if self._h is None:
+            raise BmpcError("update_system_from_device() before setup()")
+        n = self._B if self._per_instance else 1
+        def dev_ptr(M, shape, name):
+            if M is None or isinstance(M, int):
+                return M
+            ok = ((n,) + shape,) if n > 1 else (shape, (1,) + shape)
+            if tuple(M.shape) not in ok or not M.is_contiguous() or str(M.dtype) != "torch.float64" or not M.is_cuda \
+                    or M.device.index != self.device:
+                raise ValueError(f"{name} must be a contiguous float64 CUDA tensor of shape {ok[0]}")
+            return M.data_ptr()
+        a = dev_ptr(Ad_ptr, (self.nx, self.nx), "Ad"); b = dev_ptr(Bd_ptr, (self.nx, self.nu), "Bd")
+        self._check(self._L.bmpc_update_system(self._h, a, b, 1))
+
     def solve(self):
         """Solve the QP batch.  mpc.py:366-375."""
         B, nu = self._B, self.nu

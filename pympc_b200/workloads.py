@@ -22,8 +22,13 @@ def point_mass():
                 Dumin=np.array([-0.2]), Dumax=np.array([0.2]))
 
 
+# cart-pole constants of the inverted-pendulum example: cart mass M, pole mass m, cart friction b, pole friction ftheta, pole
+# length l, gravity g, sampling time Ts
+CARTPOLE = (0.5, 0.2, 0.1, 0.1, 0.3, 9.81, 50e-3)
+
+
 def pendulum():
-    M, m, b, ftheta, l, g, Ts = 0.5, 0.2, 0.1, 0.1, 0.3, 9.81, 50e-3
+    M, m, b, ftheta, l, g, Ts = CARTPOLE
     Ac = np.array([[0, 1, 0, 0],
                    [0, -b / M, -(g * m) / M, (ftheta * m) / M],
                    [0, 0, 0, 1],
@@ -47,6 +52,60 @@ def pendulum_random(batch, seed=0):
     Xref = np.zeros((batch, 4))
     Xref[:, 0] = rng.uniform(-0.5, 0.3, batch)
     return X0, Xref
+
+
+def _ops(X):
+    """(sin, cos, stack) for numpy arrays or torch tensors"""
+    if type(X).__module__.startswith("torch"):
+        import torch
+        return torch.sin, torch.cos, torch.stack
+    return np.sin, np.cos, np.stack
+
+
+def _cartpole_terms(X, U):
+    M, m, b, ft, l, g, _ = CARTPOLE
+    sin, cos, stack = _ops(X)
+    v, th, om = X[..., 1], X[..., 2], X[..., 3]
+    F = U[..., 0] if U.ndim == X.ndim else U
+    s, c = sin(th), cos(th)
+    D = M + m * s * s                                  # effective mass of the cart
+    f = F - b * v                                      # force minus cart friction
+    N1 = m * l * s * om * om - m * g * s * c + m * ft * c * om + f
+    N3 = (M + m) * (g * s - ft * om) - m * l * om * om * s * c - f * c
+    return stack, v, om, s, c, D, f, N1, N3
+
+
+def cartpole_rhs(X, U):
+    """Nonlinear cart-pole whose linearisation at the upright equilibrium is pendulum()'s model — the plant the inverted-pendulum
+    example simulates in closed loop.  Batched: X [B,4] = (cart position, cart velocity v, pole angle theta from upright, angular
+    velocity omega), U [B,1] or [B] = force on the cart; returns dX/dt [B,4].  Constants: CARTPOLE.  numpy arrays or torch tensors."""
+    l = CARTPOLE[4]
+    stack, v, om, s, c, D, f, N1, N3 = _cartpole_terms(X, U)
+    return stack([v, N1 / D, om, N3 / (l * D)], -1)
+
+
+def cartpole_linearised(X, U, Ts=CARTPOLE[6]):
+    """Euler-discretised Jacobians of cartpole_rhs about each instance's (x, u): Ad = I + Ts df/dx [B,4,4], Bd = Ts df/du [B,4,1] —
+    the model a successive-linearisation MPC hands to MPCController.update_system at every sample.  At the upright equilibrium
+    (x = 0, u = 0) they are pendulum()'s Ad and Bd.  numpy arrays or torch tensors (the result lives where X does)."""
+    M, m, b, ft, l, g, _ = CARTPOLE
+    stack, v, om, s, c, D, f, N1, N3 = _cartpole_terms(X, U)
+    dD = 2.0 * m * s * c                               # dD/dtheta
+    av, aw = N1 / D, N3 / (l * D)
+    # cart acceleration av = N1 / D
+    dav_dv, dav_dom, dav_dF = -b / D, (2.0 * m * l * s * om + m * ft * c) / D, 1.0 / D
+    dav_dth = (m * l * c * om * om - m * g * (c * c - s * s) - m * ft * s * om - av * dD) / D
+    # angular acceleration aw = N3 / (l D)
+    daw_dv, daw_dom, daw_dF = b * c / (l * D), (-(M + m) * ft - 2.0 * m * l * om * s * c) / (l * D), -c / (l * D)
+    daw_dth = ((M + m) * g * c - m * l * om * om * (c * c - s * s) + f * s - aw * l * dD) / (l * D)
+    z = v * 0.0
+    o = z + 1.0
+    Ad = stack([stack([o, z + Ts, z, z], -1),
+                stack([z, 1.0 + Ts * dav_dv, Ts * dav_dth, Ts * dav_dom], -1),
+                stack([z, z, o, z + Ts], -1),
+                stack([z, Ts * daw_dv, Ts * daw_dth, 1.0 + Ts * daw_dom], -1)], -2)
+    Bd = stack([z, Ts * dav_dF, z, Ts * daw_dF], -1)[..., None]
+    return Ad, Bd
 
 
 def mimo():
