@@ -30,11 +30,23 @@ def build(force=False, verbose=False):
     return LIB
 
 
-def add_shape(nx, nu, Np, Nc=None):
-    """Register one more compile-time fast-path shape (nu must be 1, Nc <= Np, default Nc = Np) and rebuild."""
+TPI_DOMAIN = "fast-path shapes need nu == 1, nx <= 13, Np*nx <= 128, Np < 32, 1 <= Nc <= Np"
+
+
+def tpi_shape_supported(nx, nu, Np, Nc=None):
+    """True when the single-input fast path (thread-per-instance ADMM + Riccati polish, csrc/bmpc_tpi.cuh) can hold the shape:
+    nu == 1; Np*nx <= 128 and Np < 32 (the register-resident sweeps); nx <= 13 (a stage's working set is one code word of
+    2 nx + 6 bits, at most 32).  Every such shape also fits the polish's shared memory with at least one warp per CTA.
+    Other shapes run on the team kernels."""
     Nc = Np if Nc is None else Nc
-    if nu != 1 or Np * nx > 128 or Np >= 32 or not (1 <= Nc <= Np):
-        raise ValueError("fast-path shapes need nu == 1, Np*nx <= 128, Np < 32, 1 <= Nc <= Np")
+    return nu == 1 and 1 <= nx <= 13 and Np * nx <= 128 and Np < 32 and 1 <= Nc <= Np
+
+
+def add_shape(nx, nu, Np, Nc=None):
+    """Register one more compile-time fast-path shape (tpi_shape_supported, default Nc = Np) and rebuild."""
+    Nc = Np if Nc is None else Nc
+    if not tpi_shape_supported(nx, nu, Np, Nc):
+        raise ValueError(TPI_DOMAIN)
     line = f"BMPC_TPI_SHAPE({nx}, {nu}, {Np}, {Nc})"
     txt = open(SHAPES).read()
     if line not in txt:
@@ -47,8 +59,8 @@ def jit_shape(nx, nu, Np, Nc=None, verbose=False):
     (nx, 1, Np, Nc) and return its path: lets a controller of ANY single-input shape run on the thread-per-instance kernels
     without editing csrc/tpi_shapes.inc.  Raises on shapes the fast path cannot hold or when nvcc is not available."""
     Nc = Np if Nc is None else Nc
-    if nu != 1 or Np * nx > 128 or Np >= 32 or not (1 <= Nc <= Np):
-        raise ValueError("fast-path shapes need nu == 1, Np*nx <= 128, Np < 32, 1 <= Nc <= Np")
+    if not tpi_shape_supported(nx, nu, Np, Nc):
+        raise ValueError(TPI_DOMAIN)
     jdir = os.path.join(_HERE, "_jit"); os.makedirs(jdir, exist_ok=True)
     tag = f"{nx}_{nu}_{Np}_{Nc}"
     inc = os.path.join(jdir, f"shape_{tag}.inc"); lib = os.path.join(jdir, f"libbmpc_{tag}.so")

@@ -597,7 +597,8 @@ __global__ void __launch_bounds__(32) k_tpi_admm(const __grid_constant__ TpiAdmm
 
 // ------------------------------------------------------------------------------------------------
 // K5 + K6 of the fast path: persistent, work-stealing Riccati polish (bmpc_tpi.cuh, second generation).
-// One CTA per SM, TPI_POL_WARPS warps per CTA (as many as the gain workspace lets reside), every warp on its own: it
+// One CTA per SM, TpiPolLayout<S>::warps warps per CTA (as many as the gain workspaces let reside, at most TPI_POL_WARPS), every
+// warp on its own: it
 //   phase A  steals chunks of 32 instances off a cursor and runs capA active-set refinements on them (a warm solve: ONE, from
 //            the stored working sets shifted by one stage); lanes that verified publish u*, U, status, v*; the others store
 //            their updated working sets and enter a device-side queue;
@@ -620,7 +621,13 @@ struct TpiPolArgs {
     int cand_warm;                       // 1: an unverified instance hands its last candidate to the ADMM rounds when that candidate is sane
     unsigned char* codes; int code_stride;   // per instance: Np working-set codes + the multiplier scale (double) of the last refinement
 };
-constexpr int TPI_POL_WARPS = 7;
+constexpr int TPI_POL_WARPS = 7;                 // warps per CTA of k_tpi_pol when their workspaces fit (the pendulum: 230 720 B)
+constexpr size_t TPI_POL_SMEM_MAX = 232448;      // dynamic shared memory a CTA can opt into on sm_90 (227 KB)
+
+// bytes of one instance's working-set record in global memory: Np code words (2 bytes up to nx = 5, else 4) rounded up to 8,
+// then the multiplier scale (double) of the last refinement.  Host-side twin of TpiPolLayout<S>::code_stride (bmpc_create
+// sizes the records of a handle from its dims before a fast-path entry is chosen)
+static constexpr int tpi_code_stride(int nx, int Np) { return ((Np * (2 * nx + 6 <= 16 ? 2 : 4) + 7) & ~7) + 8; }
 
 template <class S>
 struct TpiPolLayout {
@@ -629,7 +636,12 @@ struct TpiPolLayout {
     static constexpr size_t gain_bytes = (size_t)GROWS * TPI_STR * 8;
     static constexpr size_t code_bytes = (((size_t)S::Np * 32 * sizeof(CT)) + 15) & ~(size_t)15;
     static constexpr size_t per_warp = gain_bytes + code_bytes;
+    // as many warps per CTA as their workspaces fit in shared memory, at most TPI_POL_WARPS (one CTA per SM)
+    static constexpr int warps = (int)(TPI_POL_SMEM_MAX / per_warp < (size_t)TPI_POL_WARPS ? TPI_POL_SMEM_MAX / per_warp : (size_t)TPI_POL_WARPS);
+    static_assert(warps >= 1, "fast-path polish: one warp's workspace exceeds the shared memory of a CTA");
+    static constexpr size_t smem = per_warp * warps;                         // dynamic shared memory of one CTA
     static constexpr int code_stride = (int)(((S::Np * sizeof(CT) + 7) & ~(size_t)7) + 8);   // bytes per instance in global memory
+    static_assert(code_stride == tpi_code_stride(S::nx, S::Np), "record size");
     static constexpr int VROWS = S::MT - 1;                                 // TPI rows of v without the spurious last row
     static_assert(VROWS <= GROWS, "slot layout");
 };
@@ -819,7 +831,7 @@ __global__ void k_tpi_fill_view(BmpcSysOff o, const double* __restrict__ sys, si
 }
 
 template <class S, bool TV, bool PERINST>
-__global__ void __launch_bounds__(TPI_POL_WARPS * 32, 1) k_tpi_pol(const __grid_constant__ TpiPolParams<S> P, BmpcInst I, TpiPolArgs A) {
+__global__ void __launch_bounds__(TpiPolLayout<S>::warps * 32, 1) k_tpi_pol(const __grid_constant__ TpiPolParams<S> P, BmpcInst I, TpiPolArgs A) {
     using L = TpiPolLayout<S>; using CT = typename TpiCode<S>::type;
     extern __shared__ double smem[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -845,7 +857,7 @@ __global__ void __launch_bounds__(TPI_POL_WARPS * 32, 1) k_tpi_pol(const __grid_
         atomicMax((unsigned long long*)(A.counts + BMPC_CNT_T1), bmpc_globaltimer());
         if (A.epoch == 0) return;
         __threadfence_system();                 // this warp's u* stores (to peers / to mapped host memory too) before its exit count
-        if (atomicAdd(A.counts + BMPC_CNT_EXIT, 1) == (int)(gridDim.x * TPI_POL_WARPS) - 1) {
+        if (atomicAdd(A.counts + BMPC_CNT_EXIT, 1) == (int)(gridDim.x * L::warps) - 1) {          // (launch_tpi_pol: L::warps per CTA)
             // last warp out: every counter of the launch is final.
             __threadfence();
             volatile int32_t* src = (volatile int32_t*)A.counts; volatile int32_t* dst = (volatile int32_t*)A.host_counts;
@@ -1066,6 +1078,7 @@ struct bmpc_handle {
     long long* gflags = nullptr; BmpcPeerFlags gpeers = {}; int g_npeer = 0, g_rank = 0, g_world = 1;   // K6 arrival flags
     long long g_epoch = 0, g_done_epoch = 0;       // one epoch per solve while flags are bound; the last epoch whose arrival is complete
     int32_t* queue = nullptr; unsigned char* codes = nullptr;        // phase-B queue and stored working sets of the fast-path polish
+    int code_stride = 0;                                             // bytes per instance of codes
     int32_t* h_count = nullptr;                                      // pinned, mapped
     int epoch = 0, spin_epoch = 0;                                   // launch epochs of the fast-path kernel's host notification
     cudaEvent_t ev[4];
@@ -1133,20 +1146,21 @@ static void launch_tpi_pol(bmpc_handle* h, const int32_t* list, int count, int m
     A.next_list = next_list; A.counts = h->counts + BMPC_CNT * h->cpar; A.counts_next = h->counts + BMPC_CNT * (1 - h->cpar); A.queue = h->queue; A.qcap = h->cfg.batch; A.u0_out = h->I.u0; A.um1_solved = h->um1_solved;
     A.codes = h->codes; A.code_stride = L::code_stride; A.cand_warm = h->cfg.candidate_warm;
     const int nchunks = (count + 31) / 32;
-    int grid = (nchunks + TPI_POL_WARPS - 1) / TPI_POL_WARPS;
+    int grid = (nchunks + L::warps - 1) / L::warps;
     if (grid > h->sm_count) grid = h->sm_count;
     if (grid < 1) grid = 1;
-    const size_t sm = L::per_warp * TPI_POL_WARPS;
+    const size_t sm = L::smem;
+    constexpr int threads = L::warps * 32;          // the kernel's last-warp exit count assumes exactly this block size
     A.pview = h->tpi_view; A.pstride = h->cfg.batch;
     A.host_counts = h->h_count; A.epoch = h->spin_epoch;
     A.gflags = h->gflags; A.gpeers = h->gpeers; A.g_npeer = h->g_npeer; A.g_rank = h->g_rank; A.g_world = h->g_world;
     A.g_epoch = (h->gflags && h->spin_epoch && h->g_world > 1) ? h->g_epoch : 0;
     if (h->tpi_view) {
-        if (h->xref_mode) k_tpi_pol<S, true, true><<<grid, TPI_POL_WARPS * 32, sm, h->stream>>>(PP, h->I, A);
-        else k_tpi_pol<S, false, true><<<grid, TPI_POL_WARPS * 32, sm, h->stream>>>(PP, h->I, A);
+        if (h->xref_mode) k_tpi_pol<S, true, true><<<grid, threads, sm, h->stream>>>(PP, h->I, A);
+        else k_tpi_pol<S, false, true><<<grid, threads, sm, h->stream>>>(PP, h->I, A);
     } else {
-        if (h->xref_mode) k_tpi_pol<S, true, false><<<grid, TPI_POL_WARPS * 32, sm, h->stream>>>(PP, h->I, A);
-        else k_tpi_pol<S, false, false><<<grid, TPI_POL_WARPS * 32, sm, h->stream>>>(PP, h->I, A);
+        if (h->xref_mode) k_tpi_pol<S, true, false><<<grid, threads, sm, h->stream>>>(PP, h->I, A);
+        else k_tpi_pol<S, false, false><<<grid, threads, sm, h->stream>>>(PP, h->I, A);
     }
     h->stats.launches++;
 }
@@ -1204,7 +1218,7 @@ template <class S>
 static int tpi_configure_entry() {
     if (cudaFuncSetAttribute(k_tpi_admm<S, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(S::MT * TPI_STR * 8)) != cudaSuccess) return 1;
     if (cudaFuncSetAttribute(k_tpi_admm<S, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(S::MT * TPI_STR * 8)) != cudaSuccess) return 1;
-    const int sm = (int)(TpiPolLayout<S>::per_warp * TPI_POL_WARPS);
+    const int sm = (int)TpiPolLayout<S>::smem;
     if (cudaFuncSetAttribute(k_tpi_pol<S, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm) != cudaSuccess) return 1;
     if (cudaFuncSetAttribute(k_tpi_pol<S, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm) != cudaSuccess) return 1;
     if (cudaFuncSetAttribute(k_tpi_pol<S, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm) != cudaSuccess) return 1;
@@ -1428,7 +1442,8 @@ int bmpc_create(const bmpc_config* cfg, bmpc_handle** out) {
     ok &= dalloc((void**)&h->listB, sizeof(int32_t) * B);
     ok &= dalloc((void**)&h->counts, sizeof(int32_t) * 2 * BMPC_CNT);
     ok &= dalloc((void**)&h->queue, sizeof(int32_t) * B);
-    ok &= dalloc((void**)&h->codes, (size_t)B * 72);       // largest record: 32 stages x 2 bytes + 8 (Np < 32 on the fast path)
+    h->code_stride = tpi_code_stride(d.nx, d.Np);          // the record of this shape's fast-path entry (bmpc_setup checks it)
+    ok &= dalloc((void**)&h->codes, (size_t)B * h->code_stride);
     ok &= dalloc((void**)&h->ovf, sizeof(int32_t) * (size_t)B);
     ok &= dalloc((void**)&h->vprev, sizeof(double) * (size_t)B * d.mc);
     ok &= dalloc((void**)&h->lprev, sizeof(int32_t) * (size_t)B);
@@ -1442,7 +1457,7 @@ int bmpc_create(const bmpc_config* cfg, bmpc_handle** out) {
     cudaMemset(h->I.Us, 0, sizeof(double) * B * d.NU);
     cudaMemset(h->I.Ua, 0, sizeof(double) * B * d.NU);
     cudaMemset(h->queue, 0xff, sizeof(int32_t) * B);
-    cudaMemset(h->codes, 0, (size_t)B * 72);
+    cudaMemset(h->codes, 0, (size_t)B * h->code_stride);
     cudaMemset(h->counts, 0, sizeof(int32_t) * 2 * BMPC_CNT);
     cudaMemset(h->um1_alt, 0, sizeof(double) * B * d.nu);
     h->I.sys_stride = h->cfg.n_sys > 1 ? (size_t)h->o.total : 0;
@@ -1643,6 +1658,7 @@ int bmpc_setup(bmpc_handle* h, const double* Ad, const double* Bd, const double*
     }
     if (h->tpi_kind) {
         const TpiEntry& te = g_tpi_table[h->tpi_kind - 1];
+        if (te.code_stride > h->code_stride) { h->err = "fast path: working-set record larger than allocated"; return BMPC_ERR_STATE; }
         std::vector<double> hs(o.total);
         BMPC_CUDA(cudaMemcpyAsync(hs.data(), h->sys, sizeof(double) * o.total, cudaMemcpyDeviceToHost, h->stream));
         BMPC_CUDA(cudaStreamSynchronize(h->stream));

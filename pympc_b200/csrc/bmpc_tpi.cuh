@@ -368,7 +368,7 @@ inline void tpi_fill_admm(const double* sys, const BmpcSysOff& o, TpiAdmmParams<
 // Second generation.  What changed against the round-1 sweeps (profiles/ncu_r1_final_summary.txt: 23 % fp64 pipe, the
 // forward sweep spent 4 instructions on set bookkeeping per fp64 instruction):
 //  * the working sets live as ONE small code word per stage (state rows up / down, input row, delta-u row, the spurious last
-//    row) in shared memory next to the gains, and between solves as 2 bytes per stage in global memory: a warm solve reads
+//    row) in shared memory next to the gains, and between solves as 2 (nx <= 5) or 4 bytes per stage in global memory: a warm solve reads
 //    40 bytes of sets instead of the 968-byte iterate v, shifted by one stage (receding horizon: the plan of step t+1 is the
 //    tail of the plan of step t);
 //  * both sweeps are branch-free: the pin type of a stage (free / input bound / delta-u bound / spurious row) only selects
@@ -384,8 +384,10 @@ template <class S>
 struct TpiCode {
     static constexpr unsigned XUP = 0, XDN = S::nx, UUP = 2 * S::nx, UDN = UUP + 1, DUP = UUP + 2, DDN = UUP + 3, QUP = UUP + 4, QDN = UUP + 5;
     static constexpr unsigned BITS = 2 * S::nx + 6;
-    static constexpr unsigned XMASK = (1u << (2 * S::nx)) - 1u, UDMASK = 0xFu << UUP, QMASK = 0x3u << QUP;
     using type = typename std::conditional<(BITS <= 16), uint16_t, uint32_t>::type;
+    // one 32-bit word holds the sets of nx <= 13 (pympc_b200.build.tpi_shape_supported); wider states run on the team kernels
+    static_assert(BITS <= 8 * sizeof(type), "working-set code word wider than 32 bits: the fast path holds nx <= 13");
+    static constexpr unsigned XMASK = (1u << (2 * S::nx)) - 1u, UDMASK = 0xFu << UUP, QMASK = 0x3u << QUP;
 };
 
 template <class S>

@@ -384,32 +384,29 @@ class MPCController:
         (pympc_b200.build.jit_shape, cached): every (nx, 1, Np, Nc) runs on the thread-per-instance kernels, like the reference
         handles every shape uniformly (mpc.py:456-615).  Falls back to the generic team kernels with a warning if that build is
         not possible (no nvcc on this machine)."""
+        from . import build
         L = _lib.load()
         opts = self.solver_options
         wants_fast = opts.get("fast_path", 1) and not opts.get("team_threads", 0) and opts.get("polish", 1) and self.SOFT_ON and not self._per_instance
         NX, NU = (self.Np + 1) * self.nx, self.Nc * self.nu
         small = (NX + NU + (self.Nc + 1) * self.nu) <= 192 and NU <= 64          # the library's own rule for the warp-team family
-        tpi_fits = self.nu == 1 and small and self.Np * self.nx <= 128 and self.Np < 32        # the single-input kernels hold this shape
+        tpi_fits = small and build.tpi_shape_supported(self.nx, self.nu, self.Np, self.Nc)    # the single-input kernels hold this shape
         if wants_fast and int(opts.get("fast_path", 1)) >= 2 and not tpi_fits and 2 * self.nx + 10 * self.nu <= 64 \
                 and not L.bmpc_has_multi_input_fast_path(self.nx, self.nu, self.Np, self.Nc) and not os.environ.get("BMPC_NO_JIT"):
             # fast_path=2: also build the multi-input Riccati polish for this shape (and this system's sparsity pattern) on the spot
             try:
-                from . import build
                 return _lib.load(build.jit_multi_input_shape(self.nx, self.nu, self.Np, self.Nc, self.Ad, self.Bd))
             except Exception as exc:
                 warnings.warn(f"building a multi-input fast path for shape (nx={self.nx}, nu={self.nu}, Np={self.Np}, Nc={self.Nc}) failed ({exc}): "
                               "running on the generic team kernels")
                 return L
-        if not (wants_fast and self.nu == 1 and small) or L.bmpc_has_fast_path(self.nx, self.nu, self.Np, self.Nc):
-            return L
-        if self.Np * self.nx > 128 or self.Np >= 32:
-            return L
+        if not (wants_fast and tpi_fits) or L.bmpc_has_fast_path(self.nx, self.nu, self.Np, self.Nc):
+            return L                            # (a shape outside the fast path's domain runs on the team kernels)
         if os.environ.get("BMPC_NO_JIT"):
             warnings.warn(f"no compiled fast path for shape (nx={self.nx}, nu=1, Np={self.Np}, Nc={self.Nc}): running on the generic team "
                           f"kernels (about 15x slower); add it with  python -m pympc_b200.build --add-shape {self.nx},1,{self.Np},{self.Nc}")
             return L
         try:
-            from . import build
             return _lib.load(build.jit_shape(self.nx, 1, self.Np, self.Nc))
         except Exception as exc:
             warnings.warn(f"no compiled fast path for shape (nx={self.nx}, nu=1, Np={self.Np}, Nc={self.Nc}) and building one failed ({exc}): "

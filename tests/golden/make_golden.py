@@ -7,9 +7,15 @@ Closed loops use the linear plant x+ = Ad x + Bd u (README.md:59-77 pattern).
 
     python tests/golden/make_golden.py              # every fixture
     python tests/golden/make_golden.py reference    # only ref_assembly.npz and ref_on_port.npz
+    python tests/golden/make_golden.py shapes       # only shapes.npz (single-input shapes at the edges of the fast path)
 """
 import os
 import sys
+
+if sys.argv[1:] == ["shapes"]:
+    # one process per shape: single-threaded BLAS keeps them from competing and the results reproducible
+    for _v in ("OPENBLAS_NUM_THREADS", "OMP_NUM_THREADS", "MKL_NUM_THREADS"):
+        os.environ.setdefault(_v, "1")
 
 import numpy as np
 
@@ -151,7 +157,84 @@ def reference_on_port(nsteps=5):
     print("ref_on_port u", np.array(us).ravel())
 
 
+# Single-input shapes at the edges of the fast path's domain (tests/test_gpu_shapes.py, tests/test_hostemu_core.py):
+# (nx, Np, Nc, instances).  nu = 1 throughout.
+SHAPES = [(1, 31, 31, 32), (2, 29, 29, 32), (2, 31, 16, 32), (4, 25, 25, 16), (4, 31, 1, 16), (5, 17, 17, 16), (6, 21, 21, 16),
+          (8, 16, 16, 16), (13, 8, 8, 32), (14, 7, 7, 32)]
+SHAPE_STEPS = 4
+
+
+def random_system(rng, nx, nu, Np, Nc=None, eps_feas=1e3):
+    """Seeded random system: spectral radius <= 1.05, random Bd, diagonal weights, finite boxes on every row
+    (the recipe of tests/test_gpu_parity.py::_random_system)."""
+    A = rng.standard_normal((nx, nx)); A *= min(1.0, 1.05 / max(abs(np.linalg.eigvals(A))))
+    return dict(Ad=A, Bd=rng.standard_normal((nx, nu)), Np=Np, Nc=Nc or Np, Qx=np.diag(rng.uniform(0.1, 2.0, nx)),
+                QxN=np.diag(rng.uniform(0.1, 2.0, nx)), Qu=np.diag(rng.uniform(0.0, 0.5, nu)), QDu=np.diag(rng.uniform(0.05, 1.0, nu)),
+                xmin=-rng.uniform(0.5, 3.0, nx), xmax=rng.uniform(0.5, 3.0, nx), umin=-rng.uniform(0.3, 2.0, nu),
+                umax=rng.uniform(0.3, 2.0, nu), Dumin=-rng.uniform(0.2, 1.0, nu), Dumax=rng.uniform(0.2, 1.0, nu), eps_feas=eps_feas)
+
+
+def certified(K, warm=None):
+    """Exact minimiser of the QP the reference assembled, KKT residuals < 1e-9: the ADMM -> active-set oracle, or, when it cannot
+    certify the QP, the least-distance solver (oracle/ldp.py) whose active set one primal-dual active-set solve then certifies."""
+    from types import SimpleNamespace
+    from oracle.kkt import _pdas
+    from oracle.ldp import solve_mpc
+    P, A = K.P.toarray(), K.A.toarray()
+    try:
+        return exact(K, warm)
+    except (RuntimeError, AssertionError):
+        pass
+    NX, NU = (K.Np + 1) * K.nx, K.Nc * K.nu
+    l = np.where(K.l < -1e20, -np.inf, K.l); u = np.where(K.u > 1e20, np.inf, K.u)
+    U = solve_mpc(SimpleNamespace(NX=NX, NU=NU, A=A, P=P, q=K.q, l=l, u=u))
+    X = np.linalg.solve(A[:NX, :NX], l[:NX] - A[:NX, NX:NX + NU] @ U)
+    E = np.clip(X, l[NX:2 * NX], u[NX:2 * NX]) - X                 # slack of the soft rows xmin <= X + E <= xmax
+    z = np.concatenate([X, U, E]); Az = A @ z
+    out = _pdas(P, K.q, A, l, u, Az <= l + 1e-7 * (1 + np.abs(l)), Az >= u - 1e-7 * (1 + np.abs(u)), max_steps=20)
+    assert out is not None, "least-distance fallback not certified"
+    z, y = out
+    r = kkt_residuals(P, K.q, A, l, u, z, y)
+    assert max(r.values()) < 1e-9, r
+    return z, y, r
+
+
+def shape_case(spec):
+    nx, Np, Nc, N = spec
+    rng = np.random.default_rng([2026, nx, Np, Nc])
+    c = random_system(rng, nx, 1, Np, Nc)
+    X0 = rng.uniform(1.3 * c["xmin"], 1.3 * c["xmax"], (N, nx)); Xref = 0.5 * rng.standard_normal((N, nx))
+    NX = (Np + 1) * nx
+    X = np.zeros((SHAPE_STEPS, N, nx)); U = np.zeros((SHAPE_STEPS, N)); useq = np.zeros((SHAPE_STEPS, N, Nc))
+    for b in range(N):
+        K = MPC(**dict(c, x0=X0[b], xref=Xref[b], uminus1=np.zeros(1))); K.setup(solve=False)
+        x = X0[b].copy(); um1 = np.zeros(1); warm = None
+        for t in range(SHAPE_STEPS):
+            K.update(x, um1, solve=False)
+            z, y, r = certified(K, warm); warm = (z, y)
+            X[t, b] = x; useq[t, b] = z[NX:NX + Nc]; U[t, b] = z[NX]
+            um1 = z[NX:NX + 1].copy(); x = c["Ad"] @ x + c["Bd"] @ um1
+    tag = f"{nx}_{Np}_{Nc}_"
+    out = {tag + k: np.asarray(v, float) for k, v in c.items() if k not in ("Np", "Nc")}
+    out.update({tag + "X": X, tag + "U": U, tag + "useq": useq, tag + "Xref": Xref})
+    print("shapes", spec, "u0[:3]", U[0, :3], flush=True)
+    return out
+
+
+def shapes():
+    from multiprocessing import Pool
+    with Pool(min(len(SHAPES), os.cpu_count() or 1)) as pool:
+        parts = pool.map(shape_case, sorted(SHAPES, key=lambda s: -s[0] * s[1] * s[3]))
+    out = {}
+    for p in parts:
+        out.update(p)
+    np.savez_compressed(os.path.join(OUT, "shapes.npz"), shapes=np.array(SHAPES), steps=SHAPE_STEPS, **out)
+
+
 if __name__ == "__main__":
+    if sys.argv[1:] == ["shapes"]:
+        shapes()
+        sys.exit(0)
     if sys.argv[1:] == ["reference"]:        # only the records of the reference's solver inputs (tests/test_oracle.py)
         reference_assembly(); reference_on_port()
         sys.exit(0)
@@ -162,3 +245,4 @@ if __name__ == "__main__":
     random_batch()
     variants()
     reference_assembly(); reference_on_port()
+    shapes()

@@ -203,6 +203,13 @@ extern "C" int emu_tpi2_step(int nx, int nu, int Np, int Nc, const double* sys, 
         return xref_mode ? emu_tpi2_run<TpiShape<2, 1, 20, 20>, true>(EMU_TPI2_ARGS) : emu_tpi2_run<TpiShape<2, 1, 20, 20>, false>(EMU_TPI2_ARGS);
     if (nx == 4 && nu == 1 && Np == 20 && Nc == 10)
         return xref_mode ? emu_tpi2_run<TpiShape<4, 1, 20, 10>, true>(EMU_TPI2_ARGS) : emu_tpi2_run<TpiShape<4, 1, 20, 10>, false>(EMU_TPI2_ARGS);
+    // edges of the fast path's domain (tests/golden/shapes.npz): longest horizon, Np * nx = 128, a code word of exactly 32 bits
+    if (nx == 1 && nu == 1 && Np == 31 && Nc == 31)
+        return xref_mode ? emu_tpi2_run<TpiShape<1, 1, 31, 31>, true>(EMU_TPI2_ARGS) : emu_tpi2_run<TpiShape<1, 1, 31, 31>, false>(EMU_TPI2_ARGS);
+    if (nx == 8 && nu == 1 && Np == 16 && Nc == 16)
+        return xref_mode ? emu_tpi2_run<TpiShape<8, 1, 16, 16>, true>(EMU_TPI2_ARGS) : emu_tpi2_run<TpiShape<8, 1, 16, 16>, false>(EMU_TPI2_ARGS);
+    if (nx == 13 && nu == 1 && Np == 8 && Nc == 8)
+        return xref_mode ? emu_tpi2_run<TpiShape<13, 1, 8, 8>, true>(EMU_TPI2_ARGS) : emu_tpi2_run<TpiShape<13, 1, 8, 8>, false>(EMU_TPI2_ARGS);
 #undef EMU_TPI2_ARGS
     return -100;
 }

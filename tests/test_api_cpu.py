@@ -89,9 +89,11 @@ def test_fast_path_shape_table_is_well_formed():
     import os, re
     path = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "pympc_b200", "csrc", "tpi_shapes.inc")
     shapes = [tuple(int(v) for v in m.groups()) for m in re.finditer(r"^BMPC_TPI_SHAPE\((\d+),\s*(\d+),\s*(\d+),\s*(\d+)\)", open(path).read(), re.M)]
+    from pympc_b200.build import tpi_shape_supported
     assert len(shapes) == len(set(shapes)) >= 4
     for nx, nu, Np, Nc in shapes:
         assert nu == 1 and 1 <= Nc <= Np < 32 and Np * nx <= 128, (nx, nu, Np, Nc)
+        assert tpi_shape_supported(nx, nu, Np, Nc), (nx, nu, Np, Nc)
     for s in ((4, 1, 20, 20), (2, 1, 20, 20), (4, 1, 10, 10), (4, 1, 20, 10)):
         assert s in shapes
 
@@ -102,15 +104,69 @@ def test_fast_path_table_query_and_on_demand_shape_build(bmpc_lib):
     from pympc_b200 import build
     assert bmpc_lib.bmpc_has_fast_path(4, 1, 20, 20) == 1 and bmpc_lib.bmpc_has_fast_path(4, 1, 20, 0) == 1
     assert bmpc_lib.bmpc_has_fast_path(4, 1, 20, 10) == 1 and bmpc_lib.bmpc_has_fast_path(5, 1, 17, 17) == 0
-    for bad in ((4, 2, 20, None), (8, 1, 20, None), (2, 1, 40, None), (3, 1, 10, 11)):
+    for bad in ((4, 2, 20, None), (8, 1, 20, None), (2, 1, 40, None), (3, 1, 10, 11), (14, 1, 7, 7), (16, 1, 6, 6)):
         with pytest.raises(ValueError):
             build.jit_shape(*bad)
+        with pytest.raises(ValueError):
+            build.add_shape(*bad)
     # multi-input table (thread-per-instance Riccati polish over the scalar delta-u chain): MIMO reference-governor shape compiled in
     assert bmpc_lib.bmpc_has_multi_input_fast_path(8, 4, 40, 40) == 1 and bmpc_lib.bmpc_has_multi_input_fast_path(8, 4, 40, 0) == 1
     assert bmpc_lib.bmpc_has_multi_input_fast_path(8, 4, 12, 5) == 1 and bmpc_lib.bmpc_has_multi_input_fast_path(3, 2, 10, 10) == 0
     for bad in ((12, 5, 10, None), (3, 2, 10, 11), (30, 1, 10, None)):      # working-set word: 2 nx + 10 nu <= 64 bits
         with pytest.raises(ValueError):
             build.jit_multi_input_shape(*bad)
+
+
+def _tpi_polish_layout(nx, Np):
+    """(bytes of one warp's shared workspace, bytes of an instance's working-set record, bits of a code word) of the fast-path
+    polish, restated from TpiPolLayout / TpiCode (csrc/bmpc.cu, csrc/bmpc_tpi.cuh)"""
+    bits = 2 * nx + 6
+    cw = 2 if bits <= 16 else 4
+    per_warp = Np * (nx + 2) * 33 * 8 + ((Np * 32 * cw + 15) & ~15)
+    return per_warp, ((Np * cw + 7) & ~7) + 8, bits
+
+
+def test_fast_path_shape_predicate_states_the_kernels_domain():
+    """build.tpi_shape_supported is the one statement of which single-input shapes the thread-per-instance kernels hold: every
+    shape it accepts has a code word of at most 32 bits and fits the polish's shared memory with at least one warp per CTA;
+    it rejects the shapes whose code word would not fit (nx >= 14) and everything beyond the sweeps' limits."""
+    from pympc_b200.build import tpi_shape_supported
+    accepted = [(nx, Np) for nx in range(1, 40) for Np in range(2, 40) if tpi_shape_supported(nx, 1, Np, Np)]
+    assert max(nx for nx, _ in accepted) == 13 and max(Np for _, Np in accepted) == 31
+    fewer_warps = 0
+    for nx, Np in accepted:
+        per_warp, record, bits = _tpi_polish_layout(nx, Np)
+        assert bits <= 32 and per_warp <= 232448 and Np * nx <= 128, (nx, Np)
+        fewer_warps += per_warp * 7 > 232448
+    # the shapes that need fewer than 7 warps per CTA (all of them raised at setup before); the pendulum keeps 7
+    assert fewer_warps > 0 and _tpi_polish_layout(4, 20)[0] * 7 <= 232448
+    assert _tpi_polish_layout(6, 21)[1] == 96 and _tpi_polish_layout(8, 16)[1] == 72      # records are sized per shape
+    for shape in ((1, 1, 31, 31), (2, 1, 31, 16), (4, 1, 31, 1), (6, 1, 21, 21), (8, 1, 16, 16), (13, 1, 8, 8)):
+        assert tpi_shape_supported(*shape), shape
+    for shape in ((14, 1, 7, 7), (16, 1, 6, 6), (20, 1, 5, 5), (4, 2, 20, 20), (8, 1, 17, 17), (1, 1, 32, 32), (4, 1, 10, 11),
+                  (4, 1, 10, 0)):
+        assert not tpi_shape_supported(*shape), shape
+
+
+def test_controller_builds_fast_path_only_inside_the_domain(bmpc_lib, monkeypatch):
+    """MPCController._pick_library asks for an on-demand build exactly for the supported shapes missing from the in-tree table;
+    a shape outside the domain (nx = 14) runs on the in-tree library's team kernels without one"""
+    import warnings
+    from pympc_b200 import MPCController, build
+    asked = []
+
+    def fake_jit(nx, nu, Np, Nc=None, verbose=False):
+        asked.append((nx, nu, Np, Nc))
+        raise RuntimeError("no compiler in this test")
+    monkeypatch.setattr(build, "jit_shape", fake_jit)
+    monkeypatch.delenv("BMPC_NO_JIT", raising=False)
+    for nx, Np, expect in ((14, 7, False), (13, 8, True), (4, 20, False)):
+        K = MPCController(np.eye(nx), np.ones((nx, 1)), Np=Np)
+        with warnings.catch_warnings(record=True):
+            warnings.simplefilter("always")
+            L = K._pick_library()
+        assert L is _lib.load()
+        assert (asked[-1:] == [(nx, 1, Np, Np)]) == expect, (nx, Np, asked)
 
 
 def test_output_arrays_are_reused_only_when_the_caller_dropped_them():

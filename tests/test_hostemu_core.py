@@ -490,3 +490,36 @@ def test_tpm_pattern_specialised_shape_equals_dense(monkeypatch):
     assert sum(ps > 0 for ps, _ in runs[0]) >= 6
     for (pa, Ua), (pb, Ub) in zip(*runs):
         assert pa == pb and np.max(np.abs(Ua - Ub)) < 1e-10
+
+
+@pytest.mark.parametrize("nx,Np,Nc,min_direct", [(1, 31, 31, 1.0), (8, 16, 16, 1.0), (13, 8, 8, 0.75)])
+def test_tpi_polish_at_the_edges_of_the_shape_domain(nx, Np, Nc, min_direct):
+    """The fast path's Riccati polish (tpi2_*, host build) at the edges of its shape domain — the longest horizon, Np * nx = 128 and
+    a code word of exactly 32 bits — along the golden closed loops of tests/golden/shapes.npz (make_golden.py shapes).  Like on the
+    device, a warm step starts from the stored working sets shifted one stage (8 refinements); a step it cannot verify that way takes
+    the device's straggler route: ADMM + team polish, then the working sets read off that v*.  Every plan the polish verifies equals
+    the golden to 1e-6 (1 + |u|); the team core answers the rest exactly.  At nx = 13 the active-set iteration verifies about 85 % of
+    the warm steps alone (measured), the other shapes all of them."""
+    g = golden("shapes.npz"); tag = f"{nx}_{Np}_{Nc}_"
+    cfg = {k: g[tag + k] for k in ("Ad", "Bd", "Qx", "QxN", "Qu", "QDu", "xmin", "xmax", "umin", "umax", "Dumin", "Dumax")}
+    cfg.update(Np=Np, Nc=Nc, eps_feas=float(g[tag + "eps_feas"]))
+    X, U, S, Xref = g[tag + "X"], g[tag + "U"], g[tag + "useq"], g[tag + "Xref"]
+    T, N = U.shape
+    direct = warm = 0
+    for i in range(N):
+        E = EmuSystem(cfg)
+        for t in range(T):
+            um1 = np.array([U[t - 1, i] if t > 0 else 0.0])
+            scale = 1.0 + np.max(np.abs(S[t, i]))
+            ps = 0
+            if t > 0:
+                u, ps = E.tpi2_step(X[t, i], um1, Xref[i], mode=1, max_ref=8)
+                warm += 1; direct += ps > 0
+            if ps <= 0:
+                ut, st, it, pst, res = E.solve(X[t, i], um1, Xref[i])
+                assert st == 1 and np.max(np.abs(ut - S[t, i])) < 1e-6 * scale, (i, t, st)
+                u, ps = E.tpi2_step(X[t, i], um1, Xref[i], mode=2, max_ref=8)
+                if ps <= 0:
+                    continue
+            assert np.max(np.abs(u - S[t, i])) < 1e-6 * scale, (i, t)
+    assert direct >= min_direct * warm, (direct, warm)
