@@ -74,14 +74,35 @@ def jit_shape(nx, nu, Np, Nc=None, verbose=False):
     return lib
 
 
+TPM_DOMAIN = "multi-input fast-path shapes need nu >= 1, 1 <= nx <= 13, 2 nx + 10 nu <= 64, Np <= 64, 1 <= Nc <= Np"
+
+
+def tpm_shape_supported(nx, nu, Np, Nc=None):
+    """True when the multi-input fast path (thread-per-instance Riccati polish over the scalar delta-u chain, csrc/bmpc_tpm.cuh)
+    can hold the shape:
+      * 2 nx + 10 nu <= 64: a stage's working set is one 64-bit code word (2 soft-row bits per state, 10 bits per channel);
+      * nx <= 13 and Np <= 64: the per-thread stack frame of k_tpm_pol stays at a few KB.  The cost-to-go of order nx + nu and the
+        nx x nx state map are unrolled into registers, the working sets are three arrays of Np words.  sm_90a builds: at most
+        1.5 KB up to nx = 9 and at (2,1,64,64), 2.5-3.8 KB at nx = 10-11, 4-7 KB at nx = 12-13.  From nx = 14 on, ptxas
+        falls back to 64 registers and the frame jumps to 18 KB at (14,1,7,7), 35 KB at (18,2,6,6) and 68 KB at (22,2,6,6).
+        The driver reserves a frame for every thread the GPU can hold (270 336 on an H100 SXM): 7 KB is 1.9 GB of device
+        memory, 68 KB would be 18 GB;
+      * 1 <= Nc <= Np.
+    Other shapes run on the team kernels.  (A single-input shape inside build.tpi_shape_supported takes the single-input fast path
+    instead.)"""
+    Nc = Np if Nc is None else Nc
+    return nu >= 1 and 1 <= nx <= 13 and 2 * nx + 10 * nu <= 64 and 2 <= Np <= 64 and 1 <= Nc <= Np
+
+
 def jit_multi_input_shape(nx, nu, Np, Nc=None, Ad=None, Bd=None, verbose=False):
     """Build (once; cached under pympc_b200/_jit/) a copy of the library whose multi-input fast-path table holds the shape
     (nx, nu, Np, Nc) — with the sparsity pattern of (Ad, Bd) fixed at compile time when they are given and small enough for the
-    pattern masks (the sweeps then skip the structural zeros) — and return its path."""
+    pattern masks (the sweeps then skip the structural zeros) — and return its path.  Raises on shapes outside
+    tpm_shape_supported."""
     import numpy as np
     Nc = Np if Nc is None else Nc
-    if nu < 1 or 2 * nx + 10 * nu > 64 or not (1 <= Nc <= Np):
-        raise ValueError("multi-input fast-path shapes need 2 nx + 10 nu <= 64 and 1 <= Nc <= Np")
+    if not tpm_shape_supported(nx, nu, Np, Nc):
+        raise ValueError(TPM_DOMAIN)
     line = f"BMPC_TPM_SHAPE({nx}, {nu}, {Np}, {Nc})"; tag = f"m{nx}_{nu}_{Np}_{Nc}"
     if Ad is not None and Bd is not None and nx * nx <= 64 and nx * nu <= 32:
         A = np.asarray(Ad, float).reshape(nx, nx); Bm = np.asarray(Bd, float).reshape(nx, nu)

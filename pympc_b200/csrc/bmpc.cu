@@ -300,7 +300,9 @@ __global__ void __launch_bounds__(NS >= 4 ? 768 : 512) k_admm_tile(BmpcDims d, B
     bmpc_tile_load_rows(t, d, o, sys, S.lo, S.hi, S.rho);
     for (int idx = t.tid; idx < d.nu * T; idx += t.n) { const int e = idx / d.nu, q = idx % d.nu; S.um1[idx] = I.um1[(size_t)S.inst[e] * d.nu + q]; }
     if (do_prep) {
-        double* x0 = S.r;                                              // staging: r is free until the first iteration
+        // staging: v (mc T >= nx T doubles) is free until it is loaded below.  (r, NU T doubles, was too small when Nc nu < nx and
+        // overwrote u_-1 and the other per-instance values carved behind it: g then held the wrong u_-1 term.)
+        double* x0 = S.v;
         for (int idx = t.tid; idx < d.nx * T; idx += t.n) { const int e = idx / d.nx, c = idx % d.nx; x0[idx] = I.x0[(size_t)S.inst[e] * d.nx + c]; }
         t.sync();
         bmpc_tile_prep(t, d, o, sys, S, x0, I.xref, xref_mode);

@@ -71,6 +71,10 @@ struct TpmLayout {
     static constexpr int n = S::nx + S::nu, nz = n + 3, per_stage = S::nu * nz, slots = S::Np * per_stage;
     // v* staged in a consumed stage block: sub-step j: input row at 2 j, chain row at 2 j + 1; then the nx rows of x_{k+1}
     static_assert(per_stage >= S::nx + 2 * S::nu, "stage block too small for the staged v*");
+    // the domain of pympc_b200.build.tpm_shape_supported (the code word is checked by TpmCode): wider states or longer horizons
+    // make the per-thread stack frame of k_tpm_pol grow to tens of KB
+    static_assert(S::nx >= 1 && S::nx <= 13 && S::Np >= 2 && S::Np <= 64 && S::Nc >= 1 && S::Nc <= S::Np,
+                  "multi-input fast-path shapes need nx <= 13, Np <= 64, 1 <= Nc <= Np");
 };
 
 // index of (a, b) in a packed upper triangle of order n (either order of the arguments)

@@ -391,7 +391,7 @@ class MPCController:
         NX, NU = (self.Np + 1) * self.nx, self.Nc * self.nu
         small = (NX + NU + (self.Nc + 1) * self.nu) <= 192 and NU <= 64          # the library's own rule for the warp-team family
         tpi_fits = small and build.tpi_shape_supported(self.nx, self.nu, self.Np, self.Nc)    # the single-input kernels hold this shape
-        if wants_fast and int(opts.get("fast_path", 1)) >= 2 and not tpi_fits and 2 * self.nx + 10 * self.nu <= 64 \
+        if wants_fast and int(opts.get("fast_path", 1)) >= 2 and not tpi_fits and build.tpm_shape_supported(self.nx, self.nu, self.Np, self.Nc) \
                 and not L.bmpc_has_multi_input_fast_path(self.nx, self.nu, self.Np, self.Nc) and not os.environ.get("BMPC_NO_JIT"):
             # fast_path=2: also build the multi-input Riccati polish for this shape (and this system's sparsity pattern) on the spot
             try:

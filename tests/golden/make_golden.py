@@ -8,11 +8,12 @@ Closed loops use the linear plant x+ = Ad x + Bd u (README.md:59-77 pattern).
     python tests/golden/make_golden.py              # every fixture
     python tests/golden/make_golden.py reference    # only ref_assembly.npz and ref_on_port.npz
     python tests/golden/make_golden.py shapes       # only shapes.npz (single-input shapes at the edges of the fast path)
+    python tests/golden/make_golden.py mimo_shapes  # only mimo_shapes.npz (shapes at the edges of the multi-input fast path)
 """
 import os
 import sys
 
-if sys.argv[1:] == ["shapes"]:
+if sys.argv[1:] in (["shapes"], ["mimo_shapes"]):
     # one process per shape: single-threaded BLAS keeps them from competing and the results reproducible
     for _v in ("OPENBLAS_NUM_THREADS", "OMP_NUM_THREADS", "MKL_NUM_THREADS"):
         os.environ.setdefault(_v, "1")
@@ -231,9 +232,92 @@ def shapes():
     np.savez_compressed(os.path.join(OUT, "shapes.npz"), shapes=np.array(SHAPES), steps=SHAPE_STEPS, **out)
 
 
+# Shapes at the edges of the multi-input fast path's domain (tests/test_gpu_mimo_shapes.py, tests/test_hostemu_core.py):
+# (nx, nu, Np, Nc, instances, options).  Options: "qu" a full Qu, "uref" a non-zero uref, "tv" a time-varying (Np+1, nx)
+# reference per instance and step, "pattern" the non-symmetric sparsity pattern below.
+MIMO_SHAPES = [
+    (2, 6, 12, 12, 32, ("qu", "uref")),    # 2 nx + 10 nu = 64: the code word is full, the last channel's hint bits are 62-63
+    (7, 5, 8, 4, 16, ("tv", "zeros")),     # full code word; nx nu = 35 > 32: no pattern masks, a sparse system takes the dense entry
+    (8, 4, 25, 1, 16, ("pattern",)),       # Nc = 1 with four inputs: first-block row and spurious last row on one stage
+    (3, 2, 60, 60, 16, ("tv", "uref")),    # long horizon
+    (4, 1, 40, 40, 16, ()),                # pendulum-size single-input system outside the single-input domain (Np >= 32)
+    (1, 5, 20, 10, 32, ("qu",)),           # one state, five inputs, Nc < Np
+    # the widest states of the domain (nx = 13, build.tpm_shape_supported).  They stand in for (22, 2, 6, 6) and (27, 1, 4, 4), the
+    # widest states the code word holds, whose k_tpm_pol needs a stack frame of 44-68 KB per thread; those run on the team kernels
+    (13, 2, 6, 6, 16, ()),
+    (13, 1, 10, 10, 16, ()),               # (single-input, Np nx > 128: outside the single-input domain)
+    # outside the domain: with fast_path=2 they run on the team kernels, with the same exact answers
+    (22, 2, 6, 6, 16, ()),
+    (27, 1, 4, 4, 16, ()),
+    (14, 1, 7, 7, 32, ()),                 # single-input state too wide for either fast path
+]
+MIMO_STEPS = 5
+
+
+def mimo_pattern(nx, nu):
+    """Structural non-zeros of the pattern case: a lower-Hessenberg Ad (Ad[q][b] for b <= q + 1: NOT symmetric, so a transposed
+    mask skips real terms) and a Bd with one block of two rows per channel plus one entry off that pattern"""
+    am = np.array([[b <= q + 1 for b in range(nx)] for q in range(nx)])
+    bm = np.array([[a // 2 == j for j in range(nu)] for a in range(nx)]); bm[0, nu - 1] = True
+    return am, bm
+
+
+def mimo_shape_case(spec):
+    nx, nu, Np, Nc, N, opts = spec
+    rng = np.random.default_rng([2027, nx, nu, Np, Nc])
+    c = random_system(rng, nx, nu, Np, Nc)
+    if "pattern" in opts:
+        am, bm = mimo_pattern(nx, nu)
+        A = rng.standard_normal((nx, nx)) * am; A *= min(1.0, 1.05 / max(abs(np.linalg.eigvals(A))))
+        c["Ad"] = A; c["Bd"] = rng.uniform(0.5, 1.5, (nx, nu)) * rng.choice([-1.0, 1.0], (nx, nu)) * bm
+    if "zeros" in opts:
+        c["Ad"][0, nx - 1] = c["Ad"][nx - 1, 1] = 0.0; c["Bd"][1, 0] = 0.0        # structural zeros that no mask can hold
+    if "qu" in opts:
+        M = rng.standard_normal((nu, nu))
+        c["Qu"] = 0.1 * M @ M.T / nu + np.diag(rng.uniform(0.0, 0.3, nu))
+    c["uref"] = rng.uniform(-0.3, 0.3, nu) if "uref" in opts else np.zeros(nu)
+    X0 = rng.uniform(1.3 * c["xmin"], 1.3 * c["xmax"], (N, nx)); Xr = 0.5 * rng.standard_normal((N, nx))
+    if "tv" in opts:
+        # per instance and step: the base reference on a ramp over the horizon plus a wave that moves with the step
+        ramp = np.linspace(0.4, 1.0, Np + 1)[:, None]
+        Xref = np.stack([Xr[:, None, :] * ramp[None] + 0.2 * np.sin(0.3 * (np.arange(Np + 1)[None, :, None] + t) + np.arange(nx)[None, None, :])
+                         for t in range(MIMO_STEPS)])                     # (T, N, Np+1, nx)
+    else:
+        Xref = Xr
+    NX, NU = (Np + 1) * nx, Nc * nu
+    X = np.zeros((MIMO_STEPS, N, nx)); U = np.zeros((MIMO_STEPS, N, nu)); useq = np.zeros((MIMO_STEPS, N, NU))
+    for b in range(N):
+        K = MPC(**dict(c, x0=X0[b], xref=(Xref[0, b] if "tv" in opts else Xref[b]), uminus1=np.zeros(nu))); K.setup(solve=False)
+        x = X0[b].copy(); um1 = np.zeros(nu); warm = None
+        for t in range(MIMO_STEPS):
+            K.update(x, um1, xref=(Xref[t, b] if "tv" in opts else None), solve=False)
+            z, y, r = certified(K, warm); warm = (z, y)
+            X[t, b] = x; useq[t, b] = z[NX:NX + NU]; U[t, b] = z[NX:NX + nu]
+            um1 = z[NX:NX + nu].copy(); x = c["Ad"] @ x + c["Bd"] @ um1
+    tag = f"{nx}_{nu}_{Np}_{Nc}_"
+    out = {tag + k: np.asarray(v, float) for k, v in c.items() if k not in ("Np", "Nc")}
+    out.update({tag + "X": X, tag + "U": U, tag + "useq": useq, tag + "Xref": Xref})
+    print("mimo_shapes", spec[:4], "u0[:2]", U[0, :2].ravel(), flush=True)
+    return out
+
+
+def mimo_shapes():
+    from multiprocessing import Pool
+    with Pool(min(len(MIMO_SHAPES), os.cpu_count() or 1)) as pool:
+        parts = pool.map(mimo_shape_case, sorted(MIMO_SHAPES, key=lambda s: -((s[2] + 1) * s[0] + s[3] * s[1]) ** 2 * s[4]))
+    out = {}
+    for p in parts:
+        out.update(p)
+    np.savez_compressed(os.path.join(OUT, "mimo_shapes.npz"), shapes=np.array([s[:5] for s in MIMO_SHAPES]), steps=MIMO_STEPS,
+                        pattern=np.array([s[:4] for s in MIMO_SHAPES if "pattern" in s[5]][0]), **out)
+
+
 if __name__ == "__main__":
     if sys.argv[1:] == ["shapes"]:
         shapes()
+        sys.exit(0)
+    if sys.argv[1:] == ["mimo_shapes"]:
+        mimo_shapes()
         sys.exit(0)
     if sys.argv[1:] == ["reference"]:        # only the records of the reference's solver inputs (tests/test_oracle.py)
         reference_assembly(); reference_on_port()
@@ -246,3 +330,4 @@ if __name__ == "__main__":
     variants()
     reference_assembly(); reference_on_port()
     shapes()
+    mimo_shapes()

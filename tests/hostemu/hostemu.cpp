@@ -362,6 +362,20 @@ extern "C" int emu_tpm_step(int nx, int nu, int Np, int Nc, const double* sys, c
     EMU_TPM_SHAPE(4, 1, 20, 10)
     EMU_TPM_SHAPE(3, 2, 10, 10)
     EMU_TPM_SHAPE(3, 2, 10, 6)
+    // edges of the shape domain (tests/golden/mimo_shapes.npz): full code word, Nc = 1, long horizon, nu = 1, nx = 13;
+    // EMU_TPM_PATTERN: the non-symmetric pattern of the (8, 4, 25, 1) case (lower-Hessenberg Ad), as the device compiles it
+    if (nx == 8 && nu == 4 && Np == 25 && Nc == 1 && getenv("EMU_TPM_PATTERN")) {
+        using SP = TpmSparseShape<8, 4, 25, 1, 0xffff7f3f1f0f0703ull, 0x88442219u>;
+        return xref_mode ? emu_tpm_run<SP, true>(EMU_TPM_ARGS) : emu_tpm_run<SP, false>(EMU_TPM_ARGS);
+    }
+    EMU_TPM_SHAPE(2, 6, 12, 12)
+    EMU_TPM_SHAPE(7, 5, 8, 4)
+    EMU_TPM_SHAPE(8, 4, 25, 1)
+    EMU_TPM_SHAPE(3, 2, 60, 60)
+    EMU_TPM_SHAPE(4, 1, 40, 40)
+    EMU_TPM_SHAPE(1, 5, 20, 10)
+    EMU_TPM_SHAPE(13, 2, 6, 6)
+    EMU_TPM_SHAPE(13, 1, 10, 10)
 #undef EMU_TPM_SHAPE
 #undef EMU_TPM_ARGS
     return -100;

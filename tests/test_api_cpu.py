@@ -169,6 +169,67 @@ def test_controller_builds_fast_path_only_inside_the_domain(bmpc_lib, monkeypatc
         assert (asked[-1:] == [(nx, 1, Np, Np)]) == expect, (nx, Np, asked)
 
 
+def test_multi_input_shape_predicate_states_the_kernels_domain():
+    """build.tpm_shape_supported is the one statement of which shapes the multi-input polish holds: the 64-bit working-set word
+    (2 nx + 10 nu <= 64, exactly full is fine), nx <= 13 and Np <= 64 (k_tpm_pol's stack frame), 1 <= Nc <= Np — the same bounds
+    the static_asserts of csrc/bmpc_tpm.cuh enforce on every compiled shape — and jit_multi_input_shape refuses the rest before
+    invoking nvcc"""
+    import os, re
+    from pympc_b200 import build
+    ok = build.tpm_shape_supported
+    for shape in ((2, 6, 12, 12), (7, 5, 8, 4), (12, 4, 6, 6), (13, 2, 6, 6), (13, 1, 10, 10), (8, 4, 25, 1), (3, 2, 64, 64),
+                  (1, 5, 20, 10), (4, 1, 40, 40), (8, 4, 40, 40), (8, 4, 12, 5), (1, 1, 2, 1)):
+        assert ok(*shape), shape
+    for shape in ((3, 6, 12, 12), (8, 5, 8, 4), (2, 7, 4, 4), (4, 0, 10, 10), (3, 2, 10, 11), (3, 2, 10, 0), (14, 1, 7, 7),
+                  (22, 2, 6, 6), (27, 1, 4, 4), (14, 2, 6, 6), (3, 2, 65, 65), (1, 1, 1, 1), (0, 2, 10, 10)):
+        assert not ok(*shape), shape
+        with pytest.raises(ValueError):
+            build.jit_multi_input_shape(*shape)
+    accepted = [(nx, nu, Np) for nx in range(0, 40) for nu in range(0, 8) for Np in (2, 10, 64, 65) if ok(nx, nu, Np, Np)]
+    assert all(2 * nx + 10 * nu <= 64 for nx, nu, _ in accepted)
+    assert {(2 * nx + 10 * nu) for nx, nu, _ in accepted} >= {64}
+    nx_max, np_max = max(s[0] for s in accepted), max(s[2] for s in accepted)
+    assert min(s[1] for s in accepted) == 1 and max(s[1] for s in accepted) == 6
+    hdr = open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "pympc_b200", "csrc", "bmpc_tpm.cuh")).read()
+    assert int(re.search(r"S::nx <= (\d+)", hdr).group(1)) == nx_max == 13
+    assert int(re.search(r"S::Np <= (\d+)", hdr).group(1)) == np_max == 64
+    assert re.search(r"BITS <= 64", hdr)
+
+
+def test_controller_builds_multi_input_fast_path_only_inside_the_domain(bmpc_lib, monkeypatch):
+    """with fast_path=2, MPCController._pick_library asks for an on-demand multi-input build exactly for the shapes outside the
+    single-input fast path's domain, inside build.tpm_shape_supported and missing from the in-tree table; never with fast_path=1.
+    A shape it does not build for runs on the in-tree library (team kernels)."""
+    import warnings
+    from pympc_b200 import MPCController, build
+    asked = []
+
+    def fake_jit(nx, nu, Np, Nc=None, Ad=None, Bd=None, verbose=False):
+        asked.append((nx, nu, Np, Nc))
+        raise RuntimeError("no compiler in this test")
+    monkeypatch.setattr(build, "jit_multi_input_shape", fake_jit)
+    monkeypatch.setattr(build, "jit_shape", lambda *a, **k: (_ for _ in ()).throw(RuntimeError("no compiler in this test")))
+    monkeypatch.delenv("BMPC_NO_JIT", raising=False)
+    L0 = _lib.load()
+    n_yes = 0
+    for nx in (1, 2, 4, 7, 8, 12, 13, 14, 22, 27):
+        for nu in (1, 2, 4, 5, 6, 7):
+            for Np, Nc in ((4, 4), (10, 10), (20, 10), (40, 40), (8, 1), (64, 64), (65, 65)):
+                shape = (nx, nu, Np, Nc)
+                expect = (build.tpm_shape_supported(*shape) and not build.tpi_shape_supported(*shape)
+                          and not L0.bmpc_has_multi_input_fast_path(*shape))
+                for fp in (2, 1):
+                    K = MPCController(np.eye(nx), np.ones((nx, nu)), Np=Np, Nc=Nc, fast_path=fp)
+                    del asked[:]
+                    with warnings.catch_warnings(record=True):
+                        warnings.simplefilter("always")
+                        L = K._pick_library()
+                    assert L is L0
+                    assert asked == ([shape] if expect and fp == 2 else []), (shape, fp, asked)
+                n_yes += expect
+    assert n_yes >= 40
+
+
 def test_output_arrays_are_reused_only_when_the_caller_dropped_them():
     """output() returns an array the caller owns (like the reference's fresh array per call); arrays handed out earlier are
     recycled only once nobody references them — never while the caller (or uminus1_rh) still holds them"""
@@ -260,8 +321,10 @@ def test_multi_input_shape_table_is_well_formed():
         if m:
             entries.append(tuple(int(v) for v in m.groups()) + (None, None))
     assert len(entries) >= 3
+    from pympc_b200.build import tpm_shape_supported
     for nx, nu, Np, Nc, am, bm in entries:
         assert 2 * nx + 10 * nu <= 64 and 1 <= Nc <= Np, (nx, nu, Np, Nc)
+        assert tpm_shape_supported(nx, nu, Np, Nc), (nx, nu, Np, Nc)
         if am is not None:
             assert nx * nx <= 64 and nx * nu <= 32 and am < (1 << (nx * nx)) and bm < (1 << (nx * nu))
             later_dense = [e for e in entries[entries.index((nx, nu, Np, Nc, am, bm)) + 1:] if e[:4] == (nx, nu, Np, Nc) and e[4] is None]

@@ -523,3 +523,47 @@ def test_tpi_polish_at_the_edges_of_the_shape_domain(nx, Np, Nc, min_direct):
                     continue
             assert np.max(np.abs(u - S[t, i])) < 1e-6 * scale, (i, t)
     assert direct >= min_direct * warm, (direct, warm)
+
+
+# (shape, compiled pattern, least share of warm steps the polish verifies alone from the shifted sets: measured 100 % at
+# (2,6,12,12), (4,1,40,40), (1,5,20,10), 95-98 % at the others, 55 % at (7,5,8,4))
+MIMO_EDGE = [((2, 6, 12, 12), False, 0.9), ((7, 5, 8, 4), False, 0.5), ((8, 4, 25, 1), False, 0.9), ((8, 4, 25, 1), True, 0.9),
+             ((3, 2, 60, 60), False, 0.9), ((4, 1, 40, 40), False, 0.9), ((1, 5, 20, 10), False, 0.9), ((13, 2, 6, 6), False, 0.9),
+             ((13, 1, 10, 10), False, 0.9)]
+
+
+@pytest.mark.parametrize("shape,pattern,min_direct", MIMO_EDGE,
+                         ids=["-".join(map(str, s)) + ("-pattern" if p else "") for s, p, _ in MIMO_EDGE])
+def test_tpm_polish_at_the_edges_of_the_shape_domain(monkeypatch, shape, pattern, min_direct):
+    nx, nu, Np, Nc = shape
+    if pattern:
+        assert shape == tuple(int(v) for v in golden("mimo_shapes.npz")["pattern"])
+        monkeypatch.setenv("EMU_TPM_PATTERN", "1")
+    g = golden("mimo_shapes.npz"); tag = f"{nx}_{nu}_{Np}_{Nc}_"
+    cfg = {k: g[tag + k] for k in ("Ad", "Bd", "Qx", "QxN", "Qu", "QDu", "xmin", "xmax", "umin", "umax", "Dumin", "Dumax", "uref")}
+    cfg.update(Np=Np, Nc=Nc, eps_feas=float(g[tag + "eps_feas"]))
+    X, U, S, Xref = g[tag + "X"], g[tag + "U"], g[tag + "useq"], g[tag + "Xref"]
+    T, N = U.shape[:2]
+    direct = warm = verified = 0
+    for i in range(N):
+        E = EmuSystem(cfg)
+        for t in range(T):
+            um1 = U[t - 1, i] if t > 0 else np.zeros(nu)
+            xr = Xref[i] if Xref.ndim == 2 else Xref[t, i]
+            scale = 1.0 + np.max(np.abs(S[t, i]))
+            ps = 0
+            if t > 0:
+                u, ps = E.tpm_step(X[t, i], um1, xr, mode=1, max_ref=12)
+                assert ps != -100 and ps != -101
+                warm += 1; direct += ps > 0
+            if ps <= 0:
+                ut, st, it, pst, res = E.solve(X[t, i], um1, xr)
+                assert st == 1 and np.max(np.abs(ut - S[t, i])) < 1e-6 * scale, (i, t, st)
+                u, ps = E.tpm_step(X[t, i], um1, xr, mode=2, max_ref=12, exchange_from=0)
+                E.Uplan = ut.copy()
+                if ps <= 0:
+                    continue
+            verified += 1
+            assert np.max(np.abs(u - S[t, i])) < 1e-6 * scale, (i, t, ps)
+    print(f"shape {shape}{' pattern' if pattern else ''}: polish alone on {direct} of {warm} warm steps, verified {verified} of {N * T}")
+    assert direct >= min_direct * warm, (direct, warm)

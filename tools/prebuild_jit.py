@@ -12,11 +12,20 @@ sys.path.insert(0, ROOT)
 from pympc_b200 import build  # noqa: E402
 
 if __name__ == "__main__":
-    shapes = [(3, 1, 12, 9)]                                            # test_any_single_input_shape_gets_the_fast_path
+    jobs = [(build.jit_shape, (3, 1, 12, 9))]                           # test_any_single_input_shape_gets_the_fast_path
     g = np.load(os.path.join(ROOT, "tests", "golden", "shapes.npz"))     # tests/test_gpu_shapes.py (the supported ones)
-    shapes += [(int(nx), 1, int(Np), int(Nc)) for nx, Np, Nc, _ in g["shapes"] if build.tpi_shape_supported(int(nx), 1, int(Np), int(Nc))]
-    with ThreadPoolExecutor(min(len(shapes), os.cpu_count() or 1)) as ex:
-        for lib in ex.map(lambda s: build.jit_shape(*s), shapes):
-            print(lib)
+    jobs += [(build.jit_shape, (int(nx), 1, int(Np), int(Nc))) for nx, Np, Nc, _ in g["shapes"]
+             if build.tpi_shape_supported(int(nx), 1, int(Np), int(Nc))]
     A = np.ones((3, 3)); A[2, 0] = 0.0                                  # test_multi_input_fast_path_built_on_demand_for_a_dense_system
-    print(build.jit_multi_input_shape(3, 2, 10, 6, A, np.ones((3, 2))))
+    jobs.append((build.jit_multi_input_shape, (3, 2, 10, 6, A, np.ones((3, 2)))))
+    # tests/test_gpu_mimo_shapes.py: every supported shape with its golden system (and so its sparsity pattern), and the
+    # non-symmetric pattern's shape dense as well
+    g = np.load(os.path.join(ROOT, "tests", "golden", "mimo_shapes.npz"))
+    for nx, nu, Np, Nc in (tuple(int(v) for v in s[:4]) for s in g["shapes"]):
+        if build.tpm_shape_supported(nx, nu, Np, Nc) and not build.tpi_shape_supported(nx, nu, Np, Nc):
+            tag = f"{nx}_{nu}_{Np}_{Nc}_"
+            jobs.append((build.jit_multi_input_shape, (nx, nu, Np, Nc, g[tag + "Ad"], g[tag + "Bd"])))
+    jobs.append((build.jit_multi_input_shape, tuple(int(v) for v in g["pattern"])))
+    with ThreadPoolExecutor(min(len(jobs), os.cpu_count() or 1)) as ex:
+        for lib in ex.map(lambda j: j[0](*j[1]), jobs):
+            print(lib)
