@@ -6,7 +6,8 @@
 //   k_polish     K5+K6  one team per instance: active-set polish, KKT verification, output epilogue
 //   k_finalize          status / fallback output for instances the polish never verified
 //   k_sequences         optional x/u/eps sequences and objective value (output() info, mpc.py:307-328)
-// Host side: handle management and the round loop  ADMM(first_iters) -> polish -> [ADMM(chunk) -> polish]*.
+// Host side: handle management and the round loop  ADMM(first_iters) -> polish -> [ADMM(chunk) -> polish]*, each round as
+// bmpc_rounds.cuh plans it.
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -17,6 +18,7 @@
 
 #include "../../include/bmpc.h"
 #include "bmpc_core.cuh"
+#include "bmpc_rounds.cuh"
 #include "bmpc_tpi.cuh"
 #include "bmpc_tile.cuh"
 #include "bmpc_tpm.cuh"
@@ -1056,8 +1058,7 @@ struct TpiEntry {
     int view_fields; void (*fill_view)(struct bmpc_handle* h);
     int view_ad, view_bd;              // field numbers of Ad and Bd in the per-instance parameter view (k_sys_refresh)
     int (*configure)();
-    void (*launch)(struct bmpc_handle* h, const int32_t* list, int count, int niter, int32_t* next_list, cudaEvent_t mid);
-    void (*launch_polish)(struct bmpc_handle* h, const int32_t* list, int count, int32_t* next_list);
+    void (*launch)(struct bmpc_handle* h, const int32_t* list, int count, const BmpcRoundPlan& p, int32_t* next_list);
 };
 
 // ------------------------------------------------------------------------------------------------
@@ -1102,22 +1103,13 @@ struct bmpc_handle {
     bool pending = false;              // a round is in flight and has not been retired by the host yet
     int tpi_kind = 0;                  // 0 none, else 1 + index into g_tpi_table (compiled fast-path shapes)
     void *tpi_admm_params = nullptr, *tpi_polish_params = nullptr;   // host copies of the parameter blocks
-    int tpi_pdas_steps = 8;
     double* tpi_view = nullptr;       // per-instance parameter blocks of the fast path (n_sys = batch), field-major
     bool codes_valid = false;         // the stored working sets come from a fast-path polish of the whole batch
     int tpm_kind = 0;                  // 0 none, else 1 + index into g_tpm_table (compiled multi-input fast-path shapes)
     void* tpm_params = nullptr;        // host copy of the parameter block
     double* tpm_W = nullptr; unsigned long long* tpm_rec = nullptr;   // gain rows of the resident warps, working-set records
     int tpm_W_slots = 0;               // gain slots per lane tpm_W was allocated for
-    // refinements of the first launch / of a straggler round, ADMM iterations of the first straggler round.  (12, 4, 100) was measured on
-    // the MIMO side bench with the all-at-once update in the straggler rounds too (tools/sweep_tpm_caps.sh: 13.3 ms/step at 8,6,25 ->
-    // 11.4 ms); the straggler rounds now run in exchange mode, where 12 refinements finish every straggler of the host study in the
-    // first round (all-at-once, cap 4: 54 %, three rounds for the rest) — chosen in host emulation, not yet swept on the GPU
-    int tpm_first_cap = 12, tpm_round_cap = 12, tpm_chunk = 100;
-    // cold solves: working sets read off a rough ADMM iterate need 8 - 14 refinements, not 4 (host study on 48 random MIMO starts,
-    // first polish after 25 iterations: cap 4 verifies none and the solve takes 333 iterations in 4.5 rounds, cap 12 79 %, cap 16 92 %,
-    // cap 24 all of them in the first round; after 50 iterations the same picture): every polish attempt of a cold solve gets this cap
-    int tpm_cold_cap = 24;
+    BmpcPolicy policy = {};            // round policy of the chosen kernel family (bmpc_rounds.cuh)
     // time-varying (Ad, Bd), bmpc_update_system.  Per-instance systems: every instance's condensed block carries the generation it
     // was condensed for (sys_gen[i]); bmpc_update_system moves the handle's counter ahead of all of them and k_condense_list brings
     // an instance up to date right before the first launch that reads its condensed block.
@@ -1167,40 +1159,23 @@ static void launch_tpi_pol(bmpc_handle* h, const int32_t* list, int count, int m
     h->stats.launches++;
 }
 
-// first round of a fast-path solve.  niter == 0 (warm start): ONE launch, the polish starts from the previous solution's working
-// sets shifted by one stage (measured: a few ADMM iterations do not improve that first guess, DESIGN.md); niter > 0 (cold start,
-// or first_iters set): thread-per-instance ADMM, then the polish takes its working sets from the iterate.
+// k_tpi_pol of a round, after k_tpi_admm when the plan has it (first round of a cold or first_iters solve on a shared system: the
+// polish then reads its working sets off the iterate).  Without ADMM in the round the first launch resets the instances itself.
 template <class S>
-static void launch_tpi_round(bmpc_handle* h, const int32_t* list, int count, int niter, int32_t* next_list, cudaEvent_t mid) {
-    const int grid = (count + 31) / 32;
-    const TpiAdmmParams<S>& PA = *(const TpiAdmmParams<S>*)h->tpi_admm_params;
-    const int cold = h->cold ? 1 : 0, reset = h->st.round == 0 ? 1 : 0;
-    const size_t sa = S::MT * TPI_STR * 8;
-    // (a cold solve reads its working sets off a rough ADMM iterate: twice the refinements — host study on 300 random pendulum starts,
-    // first polish after 25 iterations: 88 % verify within 8 refinements, 99 % within 16, at most 3 rounds instead of 5)
-    const int capA = 1, capB = (h->st.cold ? 2 * h->tpi_pdas_steps : h->tpi_pdas_steps) - 1;
-    if (niter > 0) {
+static void launch_tpi(bmpc_handle* h, const int32_t* list, int count, const BmpcRoundPlan& p, int32_t* next_list) {
+    if (p.admm == BMPC_ADMM_TPI) {
+        const int grid = (count + 31) / 32;
+        const TpiAdmmParams<S>& PA = *(const TpiAdmmParams<S>*)h->tpi_admm_params;
+        const int cold = h->cold ? 1 : 0;
+        const size_t sa = S::MT * TPI_STR * 8;
         if (h->xref_mode)   // one (Np+1) x nx reference per instance
-            k_tpi_admm<S, true><<<grid, 32, sa, h->stream>>>(PA, h->I, list, count, niter, cold, reset, h->counts + BMPC_CNT * h->cpar, h->um1_solved);
+            k_tpi_admm<S, true><<<grid, 32, sa, h->stream>>>(PA, h->I, list, count, p.chunk, cold, p.reset, h->counts + BMPC_CNT * h->cpar, h->um1_solved);
         else
-            k_tpi_admm<S, false><<<grid, 32, sa, h->stream>>>(PA, h->I, list, count, niter, cold, reset, h->counts + BMPC_CNT * h->cpar, h->um1_solved);
+            k_tpi_admm<S, false><<<grid, 32, sa, h->stream>>>(PA, h->I, list, count, p.chunk, cold, p.reset, h->counts + BMPC_CNT * h->cpar, h->um1_solved);
         h->stats.launches++;
-        cudaEventRecord(mid, h->stream);
-        launch_tpi_pol<S>(h, list, count, 2, capA, capB, 0, next_list);
-    } else {
-        // (this round's counters were zeroed by the previous fast-path launch, or by a memset)
-        // working sets: stored ones (shifted one stage), or — when the last solve of the batch did not go through this kernel (cold
-        // start on the team kernels) — from the iterate v
-        launch_tpi_pol<S>(h, list, count, h->codes_valid ? (h->cfg.shift_warm ? 1 : 0) : 2, capA, capB, reset, next_list);
+        cudaEventRecord(h->ev[1], h->stream);
     }
-    if (list == nullptr) h->codes_valid = true;
-}
-
-// straggler rounds: the listed instances come back from an ADMM chunk of the team kernels, working sets from their iterate
-template <class S>
-static void launch_tpi_polish_only(bmpc_handle* h, const int32_t* list, int count, int32_t* next_list) {
-    h->spin_epoch = 0;
-    launch_tpi_pol<S>(h, list, count, 2, 2, (h->st.cold ? 2 * h->tpi_pdas_steps : h->tpi_pdas_steps) - 2, 0, next_list);
+    launch_tpi_pol<S>(h, list, count, p.ws, p.capA, p.capB, p.admm == BMPC_ADMM_NONE ? p.reset : 0, next_list);
 }
 
 template <class S>
@@ -1232,8 +1207,7 @@ static int tpi_configure_entry() {
      TpiPolLayout<TpiShape<NX_, NU_, NP_, NC_>>::code_stride,                                                                \
      tpi_fill_entry<TpiShape<NX_, NU_, NP_, NC_>>, TpiPolView<TpiShape<NX_, NU_, NP_, NC_>>::NF, tpi_fill_view_entry<TpiShape<NX_, NU_, NP_, NC_>>, \
      tpi_view_field_ad<TpiShape<NX_, NU_, NP_, NC_>>(), tpi_view_field_bd<TpiShape<NX_, NU_, NP_, NC_>>(),                   \
-     tpi_configure_entry<TpiShape<NX_, NU_, NP_, NC_>>,                                                                        \
-     launch_tpi_round<TpiShape<NX_, NU_, NP_, NC_>>, launch_tpi_polish_only<TpiShape<NX_, NU_, NP_, NC_>>},
+     tpi_configure_entry<TpiShape<NX_, NU_, NP_, NC_>>, launch_tpi<TpiShape<NX_, NU_, NP_, NC_>>},
 // BMPC_TPI_SHAPES_FILE: pympc_b200.build.jit_shape() compiles a copy of the library whose table holds the one shape a controller
 // asked for (any nx, Np with nu == 1) when the in-tree table does not have it
 #ifndef BMPC_TPI_SHAPES_FILE
@@ -1611,6 +1585,10 @@ static int tpm_prepare(bmpc_handle* h, const double* hs, int kind, bool fresh) {
     return BMPC_OK;
 }
 
+static int policy_family(const bmpc_handle* h) {
+    return h->tpi_kind ? (h->tpi_view ? BMPC_FAM_TPI_VIEW : BMPC_FAM_TPI) : h->tpm_kind ? BMPC_FAM_TPM : BMPC_FAM_TEAM;
+}
+
 // per-instance systems after bmpc_update_system: bring the condensed blocks of the listed instances (nullptr: 0..count-1) up to date
 // before a launch that reads them; instances already fresh cost one CTA that leaves at once.  Returns 1 if it launched.
 static int condense_stale(bmpc_handle* h, const int32_t* list, int count, int32_t* ncount) {
@@ -1687,9 +1665,8 @@ int bmpc_setup(bmpc_handle* h, const double* Ad, const double* Bd, const double*
         int rc = tpm_prepare(h, hs.data(), tk, true);
         if (rc) return rc;
     }
-    if (h->tpm_kind) {
-        if (const char* e = getenv("BMPC_TPM_CAPS")) sscanf(e, "%d,%d,%d,%d", &h->tpm_first_cap, &h->tpm_round_cap, &h->tpm_chunk, &h->tpm_cold_cap);   // tuning knob (tools/gpu_sweep.py)
-    }
+    const bmpc_config& c = h->cfg;
+    h->policy = bmpc_make_policy(policy_family(h), c.polish, c.first_iters, c.cold_iters, c.max_iter, c.pdas_steps, c.shift_warm);
     // time-varying (Ad, Bd) on per-instance systems: H = B'P_X B + P_U is positive definite for ANY (Ad, Bd) when P_X >= 0 and
     // P_U > 0 (Qu, QDu >= 0 and one of them > 0: the difference matrix T is positive definite) — then bmpc_update_system may defer
     // the condense to the launches that need it
@@ -1782,6 +1759,7 @@ int bmpc_update_system(bmpc_handle* h, const double* Ad, const double* Bd, int o
         const int tk = tpm_eligible(h) ? tpm_match(h, hs.data()) : 0;
         h->tpm_kind = 0;
         if (tk) { rc = tpm_prepare(h, hs.data(), tk, tk != old); if (rc) return rc; }
+        h->policy.family = policy_family(h);
         h->sys_bad = false;
         return BMPC_OK;
     }
@@ -1836,8 +1814,7 @@ static void launch_admm(bmpc_handle* h, const int32_t* list, int count, int nite
     h->stats.launches++;
 }
 
-static void launch_polish(bmpc_handle* h, const int32_t* list, int count, int32_t* next_list, int32_t* next_count) {
-    const int steps = bmpc_polish_steps(h->cfg.pdas_steps, h->st.round);
+static void launch_polish(bmpc_handle* h, const int32_t* list, int count, int steps, int32_t* next_list, int32_t* next_count) {
     if (use_fallback_team(h, list, count)) {
         k_polish<false><<<count, h->fb_team, h->fb_smem_polish, h->stream>>>(h->d, h->o, h->sys, h->I, list, count, h->fb_rmax, steps, next_list, next_count, h->I.u0, nullptr, nullptr, h->cfg.candidate_warm);
     } else if (h->team == 32) {
@@ -1858,25 +1835,26 @@ static void launch_polish(bmpc_handle* h, const int32_t* list, int count, int32_
 // ---- solve = rounds of [ADMM chunk -> polish]; the host only needs the count of unfinished instances after each
 // round.  bmpc_solve enqueues the first round and returns; whoever needs results next (bmpc_output, ...) waits once,
 // and only if stragglers remain runs further rounds.  In the warm closed loop this is ONE host sync per step.
-static int enqueue_round(bmpc_handle* h) {
+static bool plan_round(const bmpc_handle* h, BmpcRoundPlan* p) {
+    const auto& st = h->st;
+    return bmpc_plan_round(h->policy, BmpcSolveState{st.round, st.total, st.cold, h->codes_valid}, p);
+}
+
+// launches the round plan p: a first round without team ADMM is one fast-path launch pair over the batch (thread-per-instance
+// kernels, throughput-optimised); the team rounds run the CTA-per-instance kernels, latency-bound on the few stragglers
+static int enqueue_round(bmpc_handle* h, const BmpcRoundPlan& p) {
     auto& st = h->st;
-    if (st.chunk > h->cfg.max_iter - st.total) st.chunk = h->cfg.max_iter - st.total;
-    // fast path (thread-per-instance kernels, throughput-optimised) for the first round; the few stragglers are
-    // latency-bound and go to the CTA-per-instance team kernels
-    const bool tpi_ok = h->tpi_kind != 0;
-    // (per-instance systems have no thread-per-instance ADMM — its matrices live in the constant bank —: their cold start and any
-    // first_iters > 0 go through the team kernels, the warm polish-only round through k_tpi_pol with per-instance parameter blocks)
-    const bool tpi = st.round == 0 && tpi_ok && h->cfg.polish && (h->tpi_view == nullptr || st.chunk == 0);
-    // multi-input fast path: a warm solve starts with the Riccati polish alone (no ADMM, no prep)
-    const bool tpm0 = st.round == 0 && h->tpm_kind != 0 && st.chunk == 0 && !h->cold;
+    st.chunk = p.chunk;
+    const bool team = p.admm == BMPC_ADMM_TEAM;
+    const bool tpi_first = !team && p.polish == BMPC_POL_TPI;     // k_tpi_pol over the batch: it zeroes the next round's counters itself
     // straggler rounds read u_-1 from the snapshot the first round took: bmpc_output may already have queued the commit of
     // this solve's u0 into um1 (speculating that the first round finishes everything)
     h->cpar ^= 1;                                        // counters of this round: the half the previous round left zeroed
     int32_t* cnt = h->counts + BMPC_CNT * h->cpar;
     h->I.um1 = st.round > 0 ? h->um1_solved : h->um1_cur;
     h->I.x0 = h->x0_cur; h->I.u0_shadow = h->um1_alt;
-    if (!tpi) {
-        if (st.round == 0 && !tpm0) {
+    if (!tpi_first) {
+        if (team && p.reset) {
             const int B = h->cfg.batch;
             k_reset<<<(B + 255) / 256, 256, 0, h->stream>>>(h->I, B);
             h->stats.launches++;
@@ -1888,36 +1866,27 @@ static int enqueue_round(bmpc_handle* h) {
         h->stats.launches += condense_stale(h, st.list, st.count, cnt + BMPC_CNT_COND);
     }
     h->spin_epoch = 0;
-    if (tpi && st.chunk == 0) { h->epoch = (h->epoch % 1000000000) + 1; h->spin_epoch = h->epoch; ((volatile int32_t*)h->h_count)[BMPC_CNT_EPOCH] = 0; }
+    if (p.admm == BMPC_ADMM_NONE && p.polish == BMPC_POL_TPI) { h->epoch = (h->epoch % 1000000000) + 1; h->spin_epoch = h->epoch; ((volatile int32_t*)h->h_count)[BMPC_CNT_EPOCH] = 0; }
     // (a warm fast-path round times itself with the global timer and reports through mapped memory: no event records in the stream)
     if (!h->spin_epoch) BMPC_CUDA(cudaEventRecord(h->ev[0], h->stream));
-    if (tpi) {
-        g_tpi_table[h->tpi_kind - 1].launch(h, st.list, st.count, st.chunk, st.nxt, h->ev[1]);
-    } else if (tpm0) {
+    if (tpi_first) {
+        g_tpi_table[h->tpi_kind - 1].launch(h, st.list, st.count, p, st.nxt);
+        h->codes_valid = true;
+    } else if (!team) {
         BMPC_CUDA(cudaEventRecord(h->ev[1], h->stream));
-        g_tpm_table[h->tpm_kind - 1].launch(h, nullptr, st.count, -1, h->tpm_first_cap, 1, st.nxt, 0);
+        g_tpm_table[h->tpm_kind - 1].launch(h, st.list, st.count, p.ws, p.cap, p.reset, st.nxt, p.exchange);
     } else {
-        // infeasible instances never pass the polish: from the third round on, look for OSQP's certificate
-        const bool chk = st.total >= 25 && st.list != nullptr;
-        if (chk) { k_snapshot<<<st.count, 128, 0, h->stream>>>(h->d, h->I, st.list, st.count, h->vprev, h->lprev); h->stats.launches++; }
-        launch_admm(h, st.list, st.count, st.chunk, st.need_prep ? 1 : 0);
+        if (p.infeas) { k_snapshot<<<st.count, 128, 0, h->stream>>>(h->d, h->I, st.list, st.count, h->vprev, h->lprev); h->stats.launches++; }
+        launch_admm(h, st.list, st.count, p.chunk, st.need_prep ? 1 : 0);
         st.need_prep = false;
-        if (chk) {
+        if (p.infeas) {
             k_infeas<<<st.count, 128, sizeof(double) * (h->d.mc + h->d.nu + 2), h->stream>>>(h->d, h->o, h->sys, h->I, st.list, st.count, h->vprev, h->lprev, 1e-4, h->I.u0, cnt);
             h->stats.launches++;
         }
         BMPC_CUDA(cudaEventRecord(h->ev[1], h->stream));
-        // stragglers of a fast-path shape: the Riccati polish (list mode) has ~3x lower latency than the team Schur polish
-        if (h->cfg.polish && tpi_ok && st.total + st.chunk <= 200)
-            g_tpi_table[h->tpi_kind - 1].launch_polish(h, st.list, st.count, st.nxt);
-        // multi-input fast-path shapes: the Riccati polish (a refinement costs about one ADMM iteration of this shape) instead of
-        // the Schur-form one, which takes over for the instances that are still open after 200 iterations (any working set)
-        else if (h->cfg.polish && h->tpm_kind && st.total + st.chunk <= 200)           // (also the first attempt of a cold start: working sets from the iterate)
-            // (first attempt of a cold solve: all-at-once updates; every straggler round: single exchanges — with the cold cap in a
-            // cold solve, whose iterate is still rough: host study on 45 cold stragglers: cap 24 finishes all of them in their first
-            // straggler round, cap 12 needs two or three)
-            g_tpm_table[h->tpm_kind - 1].launch(h, st.list, st.count, 2, st.cold ? h->tpm_cold_cap : h->tpm_round_cap, 0, st.nxt, (st.cold && st.round == 0) ? 0 : 1);
-        else if (h->cfg.polish) launch_polish(h, st.list, st.count, st.nxt, cnt);
+        if (p.polish == BMPC_POL_TPI) g_tpi_table[h->tpi_kind - 1].launch(h, st.list, st.count, p, st.nxt);
+        else if (p.polish == BMPC_POL_TPM) g_tpm_table[h->tpm_kind - 1].launch(h, st.list, st.count, p.ws, p.cap, 0, st.nxt, p.exchange);
+        else if (p.polish == BMPC_POL_SCHUR) launch_polish(h, st.list, st.count, p.cap, st.nxt, cnt);
         else { k_check_converged<<<(st.count + 255) / 256, 256, 0, h->stream>>>(h->I, st.list, st.count, h->cfg.eps_abs, h->cfg.eps_rel, st.nxt, cnt); h->stats.launches++; }
     }
     h->I.um1 = h->um1_cur;
@@ -1960,10 +1929,8 @@ static int retire_round(bmpc_handle* h, int* more) {
     st.tight += h->h_count[BMPC_CNT_TIGHT];
     if (spun && h->h_count[BMPC_CNT_TIGHT + 1] == 1) h->g_done_epoch = h->g_epoch;
     st.list = st.nxt; int32_t* tmp = st.cur; st.cur = st.nxt; st.nxt = tmp;
-    // polish mode: cumulative first_iters, 25, 50, 100, ...; pure ADMM: OSQP's check_termination = 25
-    st.chunk = h->cfg.polish ? (st.total < 25 ? 25 - st.total : st.total) : 25;
-    if (h->tpm_kind && st.total == 0 && h->cfg.polish) st.chunk = h->tpm_chunk;        // first straggler round of a multi-input fast-path solve
-    if (st.count > 0 && st.total < h->cfg.max_iter) { *more = 1; return enqueue_round(h); }
+    BmpcRoundPlan next;
+    if (st.count > 0 && plan_round(h, &next)) { *more = 1; return enqueue_round(h, next); }
     *more = 0;
     const int B = h->cfg.batch;
     if (!h->cfg.polish) {
@@ -1997,20 +1964,9 @@ int bmpc_solve(bmpc_handle* h) {
     st.list = nullptr; st.count = B; st.cur = h->listA; st.nxt = h->listB;
     st.total = 0; st.round = 0; st.need_prep = true; st.tight = 0; st.cold = h->cold;
     if (h->gflags) h->g_epoch++;                     // every rank solves in lockstep: the arrival epoch of this step
-    // first round: NO ADMM iterations on a warm fast-path solve (the previous solution's working sets are the best first guess
-    // the active-set polish can get: measured 0 vs 1..10 iterations, DESIGN.md), 10 on the team kernels; first_iters > 0 overrides
-    const bool fast = h->tpi_kind != 0 || (h->tpm_kind != 0 && !h->cold);
-    st.chunk = h->cfg.polish ? (h->cfg.first_iters > 0 ? h->cfg.first_iters : (fast ? 0 : 10)) : 25;
-    // a cold start has no active-set guess to refresh: 25 iterations at once on the fast path, so that the first polish
-    // usually verifies and the whole batch does not take the straggler route
-    if (h->cfg.polish && h->cfg.first_iters <= 0 && fast && h->cold) st.chunk = 25;
-    // team / tile kernels, cold: 10 iterations from the free response leave working sets of hundreds of rows for the Schur polish
-    // (round 1 measured 180 ms launches on the MIMO shape): iterate longer before the first attempt
-    // (multi-input fast-path shapes: the Riccati polish takes the first attempt there and copes with the iterate after 25)
-    if (h->cfg.polish && h->cfg.first_iters <= 0 && !fast && h->cold) st.chunk = h->cfg.cold_iters > 0 ? h->cfg.cold_iters : (h->tpm_kind ? 25 : 50);
-    if (h->cfg.polish && fast && h->tpi_view && !h->cold && h->cfg.first_iters > 0) st.chunk = h->cfg.first_iters;
-    if (st.chunk > h->cfg.max_iter) st.chunk = h->cfg.max_iter;
-    int rc = enqueue_round(h);
+    BmpcRoundPlan first;
+    plan_round(h, &first);                           // (the first round is always planned)
+    int rc = enqueue_round(h, first);
     if (rc) return rc;
     h->pending = true; h->solved = true; h->committed = false;
     return BMPC_OK;

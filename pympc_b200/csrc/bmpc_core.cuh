@@ -50,9 +50,9 @@ struct BmpcSysOff {
 enum { BMPC_NLEV = 11, BMPC_LEV0 = 2 };
 // polish: active-set steps that update all rows at once before the hard rows switch to single exchanges
 enum { BMPC_PDAS_FULL = 3 };
-// refinements allowed per polish attempt: the configured count in the first two rounds of a solve (every instance passes there),
-// three times as many for the instances that come back from further ADMM rounds (few, and single exchanges need the room)
-BMPC_HOSTDEV int bmpc_polish_steps(int pdas_steps, int round) { return round >= 2 ? 3 * pdas_steps : pdas_steps; }
+// the round policy of a solve (host code; bmpc_polish_steps: refinements allowed per Schur-form polish attempt), shared by everything
+// that runs the core: the library's host loop and the host emulation
+#include "bmpc_rounds.cuh"
 BMPC_HOSTDEV double bmpc_level_factor(int l) {
     const double f[BMPC_NLEV] = {0.1, 0.31622776601683794, 1.0, 3.1622776601683795, 10.0, 31.622776601683793, 100.0,
                                  316.22776601683796, 1000.0, 3162.2776601683795, 10000.0};

@@ -14,12 +14,10 @@ _NAMES = ["Ad", "Bd", "Qx", "QxN", "Qu", "QDu", "xmin", "xmax", "umin", "umax", 
 
 def build():
     src = os.path.join(_HERE, "hostemu.cpp")
-    core = os.path.join(_HERE, "..", "..", "pympc_b200", "csrc", "bmpc_core.cuh")
-    tpi = os.path.join(_HERE, "..", "..", "pympc_b200", "csrc", "bmpc_tpi.cuh")
-    tile = os.path.join(_HERE, "..", "..", "pympc_b200", "csrc", "bmpc_tile.cuh")
-    tpm = os.path.join(_HERE, "..", "..", "pympc_b200", "csrc", "bmpc_tpm.cuh")
+    csrc = os.path.join(_HERE, "..", "..", "pympc_b200", "csrc")
+    deps = [src] + [os.path.join(csrc, f) for f in ("bmpc_core.cuh", "bmpc_rounds.cuh", "bmpc_tpi.cuh", "bmpc_tile.cuh", "bmpc_tpm.cuh")]
     os.makedirs(os.path.dirname(_SO), exist_ok=True)
-    if (not os.path.exists(_SO)) or os.path.getmtime(_SO) < max(os.path.getmtime(src), os.path.getmtime(core), os.path.getmtime(tpi), os.path.getmtime(tile), os.path.getmtime(tpm)):
+    if (not os.path.exists(_SO)) or os.path.getmtime(_SO) < max(os.path.getmtime(p) for p in deps):
         subprocess.check_call(["g++", "-O2", "-shared", "-fPIC", "-Wno-unknown-pragmas", "-x", "c++", src, "-o", _SO])
     return ctypes.CDLL(_SO)
 

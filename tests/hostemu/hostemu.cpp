@@ -45,14 +45,16 @@ int emu_solve(int nx, int nu, int Np, int Nc, const double* sys, const double* x
     int* st = (int*)calloc(d.mc + rmax, sizeof(int)); int* R = st + d.mc;
     bmpc_prep(t, d, o, sys, x0, um1, xref, xref_mode, g, cc);
     if (cold) { for (int a = 0; a < d.NU; a++) x[a] = 0.0; for (int i = 0; i < d.mc; i++) v[i] = i < d.NX ? cc[i] : 0.0; }
-    int total = 0, chunk = first_iters, status = -2, psteps = 0, lvl = BMPC_LEV0, round = 0;
+    int total = 0, status = -2, psteps = 0, lvl = BMPC_LEV0;
     const double* rhov = sys + o.rho;
-    while (total < max_iter) {
-        if (chunk > max_iter - total) chunk = max_iter - total;
-        bmpc_admm(t, d, o, sys, um1, g, cc, x, v, w, xt, r, chunk, res, lvl);
+    // the rounds of the library's team kernels: chunk and polish steps from its policy (first_iters 0: the automatic first chunk)
+    const BmpcPolicy P = bmpc_make_policy(BMPC_FAM_TEAM, 1, first_iters, 0, max_iter, pdas_steps, 1);
+    BmpcRoundPlan pl;
+    for (int round = 0; bmpc_plan_round(P, BmpcSolveState{round, total, cold != 0, false}, &pl); round++) {
+        bmpc_admm(t, d, o, sys, um1, g, cc, x, v, w, xt, r, pl.chunk, res, lvl);
         lvl = bmpc_adapt_level(t, d, o, sys, um1, v, res, lvl);
-        total += chunk;
-        int ps = bmpc_polish(t, d, o, sys, um1, g, cc, v, W0, zz, murow, st, S, tt, R, U0, U, rmax, bmpc_polish_steps(pdas_steps, round++));
+        total += pl.chunk;
+        int ps = bmpc_polish(t, d, o, sys, um1, g, cc, v, W0, zz, murow, st, S, tt, R, U0, U, rmax, pl.cap);
         if (getenv("EMU_TRACE")) printf("TRACE %d %.3e %.3e %d\n", total, res[0] / fmax(res[2], 1e-12), res[1] / fmax(res[3], 1e-12), ps);
         if (ps > 0) {
             psteps += ps; status = 1;
@@ -64,8 +66,7 @@ int emu_solve(int nx, int nu, int Np, int Nc, const double* sys, const double* x
         // candidate_warm, off by default on the device too), mirrored here
         if (getenv("EMU_WARM") && ps == 0 && bmpc_admm_stalled(res, total) && (getenv("EMU_ALWAYS") || bmpc_candidate_usable(t, d, o, sys, um1, zz, murow))) bmpc_warm_from_candidate(t, d, o, sys, zz, murow, U, x, v, lvl);
         if (!getenv("EMU_NOTIGHT") && bmpc_residuals_tight(res, total)) { status = 2; for (int a = 0; a < d.NU; a++) Uout[a] = xt[a]; break; }
-        psteps += bmpc_polish_steps(pdas_steps, round - 1);
-        chunk = total < 25 ? 25 - total : total;   // 10, 15, 25, 50, 100, ...
+        psteps += pl.cap;
     }
     if (status != 1 && status != 2) {
         bool conv = res[0] <= eps_abs + eps_rel * res[2] && res[1] <= eps_abs + eps_rel * res[3];

@@ -406,8 +406,8 @@ def test_tpm_exchange_mode_finishes_the_stragglers():
 
 
 def test_multi_input_round_loop_policy_in_emulation():
-    """the multi-input fast path's round loop as bmpc.cu::enqueue_round runs it (tools/mimo_flow_study.py mirrors chunks, caps and
-    modes): cold solves finish within two rounds, warm transient solves within the first launch plus ONE straggler round, nothing
+    """the multi-input fast path's round loop with the library's own round plans (tools/mimo_flow_study.py takes chunks, caps and
+    modes from bmpc_rounds.cuh): cold solves finish within two rounds, warm transient solves within the first launch plus ONE straggler round, nothing
     falls through to the Schur-form polish (round 2's measured policy: five rounds for a cold solve, up to three straggler rounds)"""
     import sys, os
     sys.path.insert(0, os.path.join(os.path.dirname(__file__), "..", "tools"))

@@ -1,8 +1,8 @@
-"""Host emulation of the multi-input fast path's round loop (bmpc.cu::enqueue_round) on the MIMO side bench's workload, with the
-device code compiled for the host: cold solve = [tile ADMM 25 -> polish from the iterate, all-at-once updates, cap 24] then straggler
-rounds [ADMM chunk doubling the total -> polish in exchange mode, cap 24]; warm solve = [polish from the shifted sets, all-at-once,
-cap 12] then straggler rounds [ADMM 100, 100, 200 -> polish from the iterate in exchange mode, cap 12].  Prints the distribution of
-rounds per solve and how many instances would fall through to the Schur-form polish (after 200 iterations).
+"""Host emulation of the multi-input fast path's round loop on the MIMO side bench's workload, with the device code compiled for the
+host and every round's chunk, cap and update mode as the library plans it (pympc_b200/csrc/bmpc_rounds.cuh, through
+tools/round_plan.py): cold solve = [tile ADMM -> polish from the iterate] rounds; warm solve = [polish from the shifted
+sets] then straggler rounds [ADMM -> polish from the iterate].  Prints the distribution of rounds per solve and how many instances
+would fall through to the Schur-form polish.
 Usage: python tools/mimo_flow_study.py [instances] [warm steps]"""
 import os
 import sys
@@ -13,42 +13,53 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests", "hostemu"))
 from emu import EmuSystem                       # noqa: E402
+from round_plan import plan_round               # noqa: E402
 from pympc_b200.workloads import mimo           # noqa: E402
 
-COLD_CHUNK, COLD_CAP, FIRST_CAP, ROUND_CAP, WARM_CHUNK = 25, 24, 12, 12, 100      # bmpc.cu: cold chunk, tpm_cold_cap, tpm_first_cap, tpm_round_cap, tpm_chunk
+
+def _riccati_plan(r, total, cold):
+    """the library's plan of round r, or None once the Schur-form polish takes over"""
+    p = plan_round("tpm", r, total, cold)
+    return p if p is not None and p["polish"] == "tpm" else None
+
+
+def _polish(E, cfg, x, um1, p, mode):
+    return E.tpm_step(x, um1, cfg["xref"], mode=mode, max_ref=p["cap"], exchange_from=0 if p["exchange"] else -1)
 
 
 def cold_solve(E, cfg, x, um1):
     """returns (U or None when the instance would go on to the Schur-form polish, rounds, ADMM iterations)"""
-    total = 0; chunk = COLD_CHUNK; r = 0
-    while total + chunk <= 200:
-        E.admm_only(x, um1, cfg["xref"], chunk); total += chunk
+    total = 0; r = 0
+    while (p := _riccati_plan(r, total, cold=True)) is not None:
+        E.admm_only(x, um1, cfg["xref"], p["chunk"]); total += p["chunk"]
         vs = E.v.copy()
         if hasattr(E, "mcodes"):
             del E.mcodes
-        U, ps = E.tpm_step(x, um1, cfg["xref"], mode=2, max_ref=COLD_CAP, exchange_from=-1 if r == 0 else 0)
+        U, ps = _polish(E, cfg, x, um1, p, mode=2)
         r += 1
         if ps > 0:
             return U, r, total
-        E.v = vs; chunk = total
+        E.v = vs
     return None, r, total
 
 
 def warm_solve(E, cfg, x, um1, codes, plan):
+    p = _riccati_plan(0, 0, cold=False)
+    assert p["admm"] == "none" and p["ws"] == "record"
     E.mcodes, E.Uplan = codes.copy(), plan.copy(); vprev = E.v.copy()
-    U, ps = E.tpm_step(x, um1, cfg["xref"], mode=1, max_ref=FIRST_CAP)
+    U, ps = _polish(E, cfg, x, um1, p, mode=1)
     if ps > 0:
         return U, 1, 0
     E.v = vprev; E.x = plan.copy(); E.cold = 0; E.lvl = 2
-    total = 0; chunk = WARM_CHUNK; r = 1
-    while total + chunk <= 200:
-        E.admm_only(x, um1, cfg["xref"], chunk); total += chunk
+    total = 0; r = 1
+    while (p := _riccati_plan(r, total, cold=False)) is not None:
+        E.admm_only(x, um1, cfg["xref"], p["chunk"]); total += p["chunk"]
         vs = E.v.copy()
-        U, ps = E.tpm_step(x, um1, cfg["xref"], mode=2, max_ref=ROUND_CAP, exchange_from=0)
+        U, ps = _polish(E, cfg, x, um1, p, mode=2)
         r += 1
         if ps > 0:
             return U, r, total
-        E.v = vs; chunk = total
+        E.v = vs
     return None, r, total
 
 
