@@ -118,6 +118,29 @@ int bmpc_update(bmpc_handle* h, const double* x0, const double* uminus1, const d
  * BMPC_ERR_NOT_PD: bmpc_solve returns BMPC_ERR_STATE until a successful bmpc_update_system or bmpc_setup. */
 int bmpc_update_system(bmpc_handle* h, const double* Ad, const double* Bd, int on_device);
 
+/* time-varying problem data (gain scheduling, successive linearisation, derated actuator limits, tightened constraints): replace
+ * any of the arrays of bmpc_setup of an already set-up handle without a new setup.  Arguments and layout as bmpc_setup's, each with
+ * its leading n_sys dimension (n_sys = 1: one set shared by every instance; n_sys = batch: one set per instance); a NULL array keeps
+ * its current value.  on_device = 0: host pointers, 1: device pointers on this handle's device (stream-ordered; the caller keeps
+ * them unchanged until the next solve has been retired).  bmpc_update_system(h, Ad, Bd, d) is this call with the other arrays NULL.
+ * A pending solve is retired first.  Kept: the working sets, v*, the per-instance rho level, the committed u_-1, the cold/warm flag
+ * and the scalar rho the setup chose; the next bmpc_solve is a WARM solve of the QP the reference would assemble with the new arrays.
+ * The per-row rho follows the setup's rule (rows with both bounds infinite: 1e-6): a row that changes between free and bounded
+ * changes its rho, its K^-1 ladder and the fast path's row parameters.  The answer stays exact (it does not depend on rho); the
+ * staged v* of such a row may be a poor warm start, which costs iterations only.  eps_feas, soft_on, the shapes and the solver
+ * options stay as set up; u_failure (the output of an instance that fails) follows the new uref.
+ * n_sys = 1: the system is condensed again at once and checked like bmpc_setup; the fast paths' constant-bank parameters are refilled
+ * and the multi-input entry is chosen again (a QDu that stops being diagonal moves the handle to the team kernels).
+ * n_sys = batch: the arrays go into every instance's block and the fast path's parameter view; each instance is condensed again only
+ * before the first launch that reads its condensed block (a warm solve that the fast-path polish finishes alone condenses nothing).
+ * New weights decide again whether H stays positive definite for any (Ad, Bd) (host weights: Qx, QxN, Qu, QDu >= 0 and Qu or
+ * QDu > 0 on every instance); if not, or when the weights are device pointers, every instance is condensed at once and checked.
+ * Bounds and uref never affect definiteness.
+ * BMPC_ERR_NOT_PD: the handle holds the new arrays and bmpc_solve returns BMPC_ERR_STATE until a successful update or bmpc_setup. */
+int bmpc_update_problem(bmpc_handle* h, const double* Ad, const double* Bd, const double* Qx, const double* QxN,
+                        const double* Qu, const double* QDu, const double* xmin, const double* xmax, const double* umin,
+                        const double* umax, const double* Dumin, const double* Dumax, const double* uref, int on_device);
+
 /* replaces OSQP.solve (mpc.py:366-375): K3 + K4 + K5 */
 int bmpc_solve(bmpc_handle* h);
 

@@ -27,7 +27,7 @@ class BmpcStats(ctypes.Structure):
                 ("launches", ctypes.c_int32), ("infeasible", ctypes.c_int32), ("recondensed", ctypes.c_int32)]
 
 
-EXPORTS = ["bmpc_default_config", "bmpc_create", "bmpc_destroy", "bmpc_last_error", "bmpc_setup", "bmpc_update", "bmpc_update_system",
+EXPORTS = ["bmpc_default_config", "bmpc_create", "bmpc_destroy", "bmpc_last_error", "bmpc_setup", "bmpc_update", "bmpc_update_system", "bmpc_update_problem",
            "bmpc_solve", "bmpc_output", "bmpc_get_sequences", "bmpc_bind_output", "bmpc_bind_output_peers", "bmpc_bind_gather_flags",
            "bmpc_gather_arrive", "bmpc_set_stream",
            "bmpc_synchronize", "bmpc_get_stats", "bmpc_get_sys", "bmpc_get_dims", "bmpc_host_alloc",
@@ -60,6 +60,7 @@ def load(path=None):
     L.bmpc_setup.argtypes = [P] + [DP] * 13; L.bmpc_setup.restype = ctypes.c_int
     L.bmpc_update.argtypes = [P, DP, DP, DP, ctypes.c_int, ctypes.c_int]; L.bmpc_update.restype = ctypes.c_int
     L.bmpc_update_system.argtypes = [P, DP, DP, ctypes.c_int]; L.bmpc_update_system.restype = ctypes.c_int
+    L.bmpc_update_problem.argtypes = [P] + [DP] * 13 + [ctypes.c_int]; L.bmpc_update_problem.restype = ctypes.c_int
     L.bmpc_solve.argtypes = [P]; L.bmpc_solve.restype = ctypes.c_int
     L.bmpc_output.argtypes = [P, DP, DP, ctypes.c_int, ctypes.c_int]; L.bmpc_output.restype = ctypes.c_int
     L.bmpc_get_sequences.argtypes = [P, DP, DP, DP, DP, DP]; L.bmpc_get_sequences.restype = ctypes.c_int

@@ -182,29 +182,28 @@ __global__ void k_condense(BmpcDims d, BmpcSysOff o, double* sys, double rho, do
     bmpc_condense(t, d, o, sys + (size_t)blockIdx.x * o.total, rho, sigma, alpha, eps_feas, soft_on);
 }
 
-// ---- time-varying (Ad, Bd) without a new setup (bmpc_update_system)
-// k_sys_refresh: one thread per (field, instance), field-major so that the stores into the fast path's field-major parameter view
-// (TpiPolView: field f of instance i at view[f * B + i]) are coalesced.  Writes the new Ad / Bd (batch-major, row-major; either may
-// be null) into every instance's system block and, when the handle has one, into the view's Ad / Bd fields (view_ad / view_bd: field
-// numbers).  The condensed part of the block is NOT touched here: the handle's generation counter has moved past every instance's
-// stamp, and k_condense_list re-condenses an instance before the first launch that reads its condensed block.
-__global__ void k_sys_refresh(BmpcDims d, BmpcSysOff o, double* __restrict__ sys, size_t sys_stride, int B, const double* __restrict__ Ad,
-                              const double* __restrict__ Bd, double* __restrict__ view, int view_ad, int view_bd) {
-    const int nA = Ad ? d.nx * d.nx : 0, nB = Bd ? d.nx * d.nu : 0;
+// ---- time-varying problem data without a new setup (bmpc_update_problem, bmpc_update_system)
+// One input array of bmpc_setup that an update replaces: cnt doubles per system at block offset off, read from src (batch-major:
+// system i's at src[i * cnt]); view >= 0: the field number where the fast path's parameter view holds the same numbers (Ad, Bd)
+struct BmpcRefreshSeg { const double* src; int off, cnt, view; };
+struct BmpcRefreshTab { BmpcRefreshSeg seg[13]; int n; };
+// k_sys_refresh: one thread per (double of a replaced array, instance), field-major so that the stores into the fast path's
+// field-major parameter view (TpiPolView: field f of instance i at view[f * B + i]) are coalesced.  Writes the table's arrays into
+// every instance's system block and the view-held ones into the view as well.  The condensed part of the block is NOT touched here:
+// the handle's generation counter has moved past every instance's stamp, and k_condense_list re-condenses an instance before the
+// first launch that reads its condensed block.  (The view's fields derived from bounds, weights or uref are rebuilt from the raw
+// fields by k_tpi_fill_view.)
+__global__ void k_sys_refresh(double* __restrict__ sys, size_t sys_stride, int B, const __grid_constant__ BmpcRefreshTab T,
+                              double* __restrict__ view) {
     const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (idx >= (size_t)B * (nA + nB)) return;
-    const int f = (int)(idx / B), inst = (int)(idx % B);
-    double* blk = sys + (size_t)inst * sys_stride;
-    if (f < nA) {
-        const double v = Ad[(size_t)inst * nA + f];
-        blk[o.Ad + f] = v;
-        if (view) view[(size_t)(view_ad + f) * B + inst] = v;
-    } else {
-        const int e = f - nA;
-        const double v = Bd[(size_t)inst * nB + e];
-        blk[o.Bd + e] = v;
-        if (view) view[(size_t)(view_bd + e) * B + inst] = v;
-    }
+    int f = (int)(idx / B), s = 0;
+    const int inst = (int)(idx % B);
+    while (s < T.n && f >= T.seg[s].cnt) { f -= T.seg[s].cnt; s++; }
+    if (s >= T.n) return;
+    const BmpcRefreshSeg& g = T.seg[s];
+    const double v = g.src[(size_t)inst * g.cnt + f];
+    sys[(size_t)inst * sys_stride + g.off + f] = v;
+    if (view && g.view >= 0) view[(size_t)(g.view + f) * B + inst] = v;
 }
 
 // k_condense_list: K1 over the listed instances (list == nullptr: 0..count-1), one CTA each, with the rho the setup chose (read from
@@ -823,7 +822,8 @@ __device__ __forceinline__ void tpi_pol_batch(const PP& P, const BmpcInst& I, co
     __syncwarp();
 }
 
-// per-instance parameter blocks (n_sys = batch): field-major in global memory, see TpiPolView
+// per-instance parameter blocks (n_sys = batch): field-major in global memory, see TpiPolView.  tpi_fill_pol reads only the raw
+// inputs and scal: valid on a block whose condensed part is stale (after bmpc_update_problem)
 template <class S>
 __global__ void k_tpi_fill_view(BmpcSysOff o, const double* __restrict__ sys, size_t sys_stride, int B, double* __restrict__ pg) {
     const int inst = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1115,9 +1115,10 @@ struct bmpc_handle {
     // an instance up to date right before the first launch that reads its condensed block.
     int32_t* sys_gen = nullptr; int32_t sys_gen_cur = 0;
     bool sys_stale = false;            // some instance's condensed block may predate its (Ad, Bd)
-    bool sys_lazy = false;             // H is positive definite whatever (Ad, Bd) are (decided at setup): the condense may be deferred
-    bool sys_bad = false;              // the last bmpc_update_system failed the positive-definiteness check: bmpc_solve refuses
-    double* sys_stage = nullptr;       // device copy of host (Ad, Bd) for k_sys_refresh
+    bool sys_lazy = false;             // H is positive definite whatever (Ad, Bd) are (decided at setup and whenever the weights
+                                       // change): the condense may be deferred
+    bool sys_bad = false;              // the last update failed the positive-definiteness check: bmpc_solve refuses
+    double* sys_stage = nullptr;       // device copy of host arrays for k_sys_refresh: array f of all systems at sys_stage[B * o.f]
 };
 
 static std::string g_create_err;
@@ -1551,6 +1552,12 @@ static bool host_psd(const double* Q, int n) {
     }
     return diag ? nonneg : host_pd(Q, n);
 }
+// H = B'P_X B + P_U is positive definite for ANY (Ad, Bd) when P_X >= 0 and P_U > 0 (Qx, QxN, Qu, QDu >= 0 and Qu or QDu > 0: the
+// difference matrix T is positive definite); w: the weights Qx, QxN, Qu, QDu of one system, contiguous as in its block
+static bool weights_keep_h_definite(const BmpcDims& d, const double* w) {
+    const double *Qx = w, *QxN = Qx + d.nx * d.nx, *Qu = QxN + d.nx * d.nx, *QDu = Qu + d.nu * d.nu;
+    return host_psd(Qx, d.nx) && host_psd(QxN, d.nx) && host_psd(Qu, d.nu) && host_psd(QDu, d.nu) && (host_pd(Qu, d.nu) || host_pd(QDu, d.nu));
+}
 
 // multi-input fast path: the first compiled entry of the shape whose (Ad, Bd) pattern masks contain the system's (blk: system block
 // on the host, inputs at their block offsets); 0: none
@@ -1667,17 +1674,12 @@ int bmpc_setup(bmpc_handle* h, const double* Ad, const double* Bd, const double*
     }
     const bmpc_config& c = h->cfg;
     h->policy = bmpc_make_policy(policy_family(h), c.polish, c.first_iters, c.cold_iters, c.max_iter, c.pdas_steps, c.shift_warm);
-    // time-varying (Ad, Bd) on per-instance systems: H = B'P_X B + P_U is positive definite for ANY (Ad, Bd) when P_X >= 0 and
-    // P_U > 0 (Qu, QDu >= 0 and one of them > 0: the difference matrix T is positive definite) — then bmpc_update_system may defer
-    // the condense to the launches that need it
+    // time-varying problem data on per-instance systems: when the weights keep H positive definite for ANY (Ad, Bd),
+    // bmpc_update_problem may defer the condense to the launches that need it
     h->sys_lazy = false;
     if (ns > 1) {
         h->sys_lazy = true;
-        for (int si = 0; si < ns && h->sys_lazy; si++) {
-            const double* blk = in.data() + (size_t)si * o.pw;
-            h->sys_lazy = host_psd(blk + o.Qx, d.nx) && host_psd(blk + o.QxN, d.nx) && host_psd(blk + o.Qu, d.nu) && host_psd(blk + o.QDu, d.nu) &&
-                          (host_pd(blk + o.Qu, d.nu) || host_pd(blk + o.QDu, d.nu));
-        }
+        for (int si = 0; si < ns && h->sys_lazy; si++) h->sys_lazy = weights_keep_h_definite(d, in.data() + (size_t)si * o.pw + o.Qx);
         if (!h->sys_gen) BMPC_CUDA(cudaMalloc((void**)&h->sys_gen, sizeof(int32_t) * (size_t)ns));
         BMPC_CUDA(cudaMemsetAsync(h->sys_gen, 0, sizeof(int32_t) * (size_t)ns, h->stream));
     }
@@ -1724,28 +1726,36 @@ static int check_condensed(bmpc_handle* h) {
     BMPC_CUDA(cudaStreamSynchronize(h->stream));
     for (int si = 0; si < ns; si++) if (errs[si] != 0.0) {
         h->sys_bad = true;
-        h->err = "bmpc_update_system: condensed Hessian is not positive definite (Qu/QDu/Qx with the new (Ad, Bd) make the QP non-strictly convex in U)";
+        h->err = "bmpc_update_problem: condensed Hessian is not positive definite (the new weights or (Ad, Bd) make the QP non-strictly convex in U)";
         return BMPC_ERR_NOT_PD;
     }
     return BMPC_OK;
 }
 
-int bmpc_update_system(bmpc_handle* h, const double* Ad, const double* Bd, int on_device) {
+int bmpc_update_problem(bmpc_handle* h, const double* Ad, const double* Bd, const double* Qx, const double* QxN, const double* Qu,
+                        const double* QDu, const double* xmin, const double* xmax, const double* umin, const double* umax,
+                        const double* Dumin, const double* Dumax, const double* uref, int on_device) {
     if (!h) return BMPC_ERR_ARG;
-    if (!h->is_setup) { h->err = "bmpc_update_system before bmpc_setup"; return BMPC_ERR_STATE; }
-    if (on_device != 0 && on_device != 1) { h->err = "bmpc_update_system: on_device must be 0 (host) or 1 (device)"; return BMPC_ERR_ARG; }
+    if (!h->is_setup) { h->err = "bmpc_update_problem before bmpc_setup"; return BMPC_ERR_STATE; }
+    if (on_device != 0 && on_device != 1) { h->err = "bmpc_update_problem: on_device must be 0 (host) or 1 (device)"; return BMPC_ERR_ARG; }
     BMPC_CUDA(cudaSetDevice(h->cfg.device));
     if (h->pending) { int rc = finish_solve(h); if (rc) return rc; }
-    if (!Ad && !Bd) return BMPC_OK;
     const BmpcDims& d = h->d; const BmpcSysOff& o = h->o;
-    const size_t nA = (size_t)d.nx * d.nx, nB = (size_t)d.nx * d.nu;
+    // the arrays of bmpc_setup in argument order: source, block offset, doubles per system
+    const double* src[13] = {Ad, Bd, Qx, QxN, Qu, QDu, xmin, xmax, umin, umax, Dumin, Dumax, uref};
+    const int off[13] = {o.Ad, o.Bd, o.Qx, o.QxN, o.Qu, o.QDu, o.xmin, o.xmax, o.umin, o.umax, o.Dumin, o.Dumax, o.uref};
+    const int cnt[13] = {d.nx * d.nx, d.nx * d.nu, d.nx * d.nx, d.nx * d.nx, d.nu * d.nu, d.nu * d.nu, d.nx, d.nx, d.nu, d.nu, d.nu, d.nu, d.nu};
+    bool any = false;
+    for (int f = 0; f < 13; f++) any = any || src[f];
+    if (!any) return BMPC_OK;
+    const bool model = Ad || Bd, weights = Qx || QxN || Qu || QDu;
     if (h->cfg.n_sys <= 1) {
         // shared system: eager.  New inputs into the block, K1 with the kept rho, the check of bmpc_setup, then everything that was
         // derived from the condensed block on the host: the fast paths' constant-bank parameters and the choice of the multi-input entry
-        // (a pattern that leaves the compiled masks must not be answered by a kernel that skips those entries)
+        // (a pattern that leaves the compiled masks, or a QDu that stops being diagonal, must not be answered by k_tpm_pol)
         const cudaMemcpyKind kind = on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
-        if (Ad) BMPC_CUDA(cudaMemcpyAsync(h->sys + o.Ad, Ad, sizeof(double) * nA, kind, h->stream));
-        if (Bd) BMPC_CUDA(cudaMemcpyAsync(h->sys + o.Bd, Bd, sizeof(double) * nB, kind, h->stream));
+        for (int f = 0; f < 13; f++)
+            if (src[f]) BMPC_CUDA(cudaMemcpyAsync(h->sys + off[f], src[f], sizeof(double) * cnt[f], kind, h->stream));
         k_condense_list<<<1, 256, 0, h->stream>>>(d, o, h->sys, 0, nullptr, 1, nullptr, 0, h->cfg.sigma, h->cfg.alpha, h->cfg.eps_feas,
                                                   h->cfg.soft_on, nullptr);
         BMPC_CUDA(cudaGetLastError());
@@ -1763,29 +1773,57 @@ int bmpc_update_system(bmpc_handle* h, const double* Ad, const double* Bd, int o
         h->sys_bad = false;
         return BMPC_OK;
     }
-    // per-instance systems: the new matrices go into every block and into the fast path's parameter view; the condense is deferred
+    // per-instance systems: the new arrays go into every block and into the fast path's parameter view; the condense is deferred
     // to the launches that read a condensed block (condense_stale) — unless H may lose definiteness, then all of it now + the check
     const int B = h->cfg.batch;
-    const double *dA = Ad, *dB = Bd;
-    if (!on_device) {
-        if (!h->sys_stage) BMPC_CUDA(cudaMalloc((void**)&h->sys_stage, sizeof(double) * (size_t)B * (nA + nB)));
-        if (Ad) { BMPC_CUDA(cudaMemcpyAsync(h->sys_stage, Ad, sizeof(double) * B * nA, cudaMemcpyHostToDevice, h->stream)); dA = h->sys_stage; }
-        if (Bd) { BMPC_CUDA(cudaMemcpyAsync(h->sys_stage + B * nA, Bd, sizeof(double) * B * nB, cudaMemcpyHostToDevice, h->stream)); dB = h->sys_stage + B * nA; }
-    }
     const TpiEntry* te = h->tpi_kind ? &g_tpi_table[h->tpi_kind - 1] : nullptr;
-    const size_t n = (size_t)B * ((Ad ? nA : 0) + (Bd ? nB : 0));
-    k_sys_refresh<<<(unsigned)((n + 255) / 256), 256, 0, h->stream>>>(d, o, h->sys, h->I.sys_stride, B, dA, dB, h->tpi_view,
-                                                                      te ? te->view_ad : 0, te ? te->view_bd : 0);
+    if (!on_device && !h->sys_stage) BMPC_CUDA(cudaMalloc((void**)&h->sys_stage, sizeof(double) * (size_t)B * o.pw));
+    BmpcRefreshTab T = {}; size_t per = 0;
+    bool view_fill = false;                              // an array the view holds only through derived fields (k_tpi_fill_view)
+    for (int f = 0; f < 13; f++) {
+        if (!src[f]) continue;
+        const double* s = src[f];
+        if (!on_device) {
+            BMPC_CUDA(cudaMemcpyAsync(h->sys_stage + (size_t)B * off[f], s, sizeof(double) * B * cnt[f], cudaMemcpyHostToDevice, h->stream));
+            s = h->sys_stage + (size_t)B * off[f];
+        }
+        const int view = !te ? -1 : f == 0 ? te->view_ad : f == 1 ? te->view_bd : -1;
+        view_fill = view_fill || (te && f >= 2);
+        T.seg[T.n++] = BmpcRefreshSeg{s, off[f], cnt[f], view};
+        per += (size_t)cnt[f];
+    }
+    const size_t n = (size_t)B * per;
+    k_sys_refresh<<<(unsigned)((n + 255) / 256), 256, 0, h->stream>>>(h->sys, h->I.sys_stride, B, T, h->tpi_view);
     BMPC_CUDA(cudaGetLastError());
+    if (view_fill) { te->fill_view(h); BMPC_CUDA(cudaGetLastError()); }
     h->sys_gen_cur++; h->sys_stale = true;
-    if (!h->sys_lazy) {
+    // definiteness depends on the weights alone: new host weights decide the deferral again (every instance, with the arrays this
+    // call kept: read back from the blocks); device weights are condensed and checked at once
+    bool check = model && !h->sys_lazy;
+    if (weights && on_device) { h->sys_lazy = false; check = true; }
+    else if (weights) {
+        const int nw = o.xmin - o.Qx;                     // Qx, QxN, Qu, QDu are contiguous in the block
+        std::vector<double> w((size_t)B * nw);
+        BMPC_CUDA(cudaMemcpy2DAsync(w.data(), sizeof(double) * nw, h->sys + o.Qx, sizeof(double) * h->I.sys_stride, sizeof(double) * nw, B,
+                                    cudaMemcpyDeviceToHost, h->stream));
+        BMPC_CUDA(cudaStreamSynchronize(h->stream));
+        h->sys_lazy = true;
+        for (int si = 0; si < B && h->sys_lazy; si++) h->sys_lazy = weights_keep_h_definite(d, w.data() + (size_t)si * nw);
+        check = !h->sys_lazy;
+    }
+    if (check) {
         condense_stale(h, nullptr, B, nullptr);
         BMPC_CUDA(cudaGetLastError());
         int rc = check_condensed(h);
         if (rc) return rc;
     }
-    h->sys_bad = false;
+    // (bounds and uref alone leave definiteness as it was: a handle refused after a failed update stays refused)
+    if (check || h->sys_lazy) h->sys_bad = false;
     return BMPC_OK;
+}
+
+int bmpc_update_system(bmpc_handle* h, const double* Ad, const double* Bd, int on_device) {
+    return bmpc_update_problem(h, Ad, Bd, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, on_device);
 }
 
 static bool use_fallback_team(const bmpc_handle* h, const int32_t* list, int count) {
@@ -1955,7 +1993,7 @@ static int finish_solve(bmpc_handle* h) {
 int bmpc_solve(bmpc_handle* h) {
     if (!h) return BMPC_ERR_ARG;
     if (!h->is_setup) { h->err = "bmpc_solve before bmpc_setup"; return BMPC_ERR_STATE; }
-    if (h->sys_bad) { h->err = "bmpc_solve after a failed bmpc_update_system (condensed Hessian not positive definite): update the system again or set up anew"; return BMPC_ERR_STATE; }
+    if (h->sys_bad) { h->err = "bmpc_solve after a failed bmpc_update_system / bmpc_update_problem (condensed Hessian not positive definite): update again or set up anew"; return BMPC_ERR_STATE; }
     BMPC_CUDA(cudaSetDevice(h->cfg.device));
     if (h->pending) { int rc = finish_solve(h); if (rc) return rc; }
     const int B = h->cfg.batch;

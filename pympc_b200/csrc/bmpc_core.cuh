@@ -124,6 +124,13 @@ BMPC_HD void bmpc_gemv(Team& t, const double* M, int ld, int nrows, const double
 
 // ------------------------------------------------------------------------------------------------
 // Row helpers
+// per-row rho of a constraint row with bounds [lo, hi]: rows with both bounds infinite get rho_min like OSQP, the others the
+// scalar rho (bmpc_condense; the fast path's fill applies it to the raw bounds, tpi_fill_pol)
+BMPC_HOSTDEV double bmpc_row_rho(double lo, double hi, double rho) {
+    const bool free_row = (lo < -1e29) && (hi > 1e29);
+    return free_row ? 1e-6 : rho;
+}
+
 BMPC_HD void bmpc_row_bounds(const BmpcDims& d, const double* lo0, const double* hi0, const double* um1, int i,
                              double& lo, double& hi) {
     lo = lo0[i]; hi = hi0[i];
@@ -286,8 +293,7 @@ BMPC_HD void bmpc_condense(Team& t, const BmpcDims& d, const BmpcSysOff& o, doub
         else if (i < NX + NU) { lo = sys[o.umin + (i - NX) % nu]; hi = sys[o.umax + (i - NX) % nu]; }
         else { int r = i - NX - NU; lo = sys[o.Dumin + r % nu]; hi = sys[o.Dumax + r % nu]; }
         lo0[i] = lo; hi0[i] = hi;
-        bool free_row = (lo < -1e29) && (hi > 1e29);
-        rhov[i] = free_row ? 1e-6 : rho;
+        rhov[i] = bmpc_row_rho(lo, hi, rho);
     }
     t.sync();
     // K = H + sigma I + Bcal' Rx Bcal + Ru + D' Rd D

@@ -682,22 +682,27 @@ BMPC_HD unsigned tpi2_shifted_code(const typename TpiCode<S>::type* stored, int 
     return c;
 }
 
+// The polish parameters of one system.  Reads only the system's inputs (Ad .. uref) and scal[RHO], scal[RHOE], never the condensed
+// arrays: the rows' bounds are the raw bounds (lo0 / hi0 copy them) and a row's rho follows the condense's rule (bmpc_row_rho).
+// So the fill stays valid on a block whose condensed part predates its inputs (per-instance systems after bmpc_update_problem,
+// k_tpi_fill_view), and gives bit for bit the block a fill from a freshly condensed system gives.
 template <class S>
 BMPC_HOSTDEV void tpi_fill_pol(const double* sys, const BmpcSysOff& o, TpiPolParams<S>& P) {
-    constexpr int nx = S::nx, NU = S::NU, NX = S::NX;
+    constexpr int nx = S::nx;
     for (int i = 0; i < nx * nx; i++) { P.Ad[i] = sys[o.Ad + i]; P.Qx[i] = sys[o.Qx + i]; P.QxN[i] = sys[o.QxN + i]; }
     for (int i = 0; i < nx; i++) P.Bd[i] = sys[o.Bd + i];
-    const double rho_e = sys[o.scal + BMPC_S_RHOE];
+    const double rho_e = sys[o.scal + BMPC_S_RHOE], rho = sys[o.scal + BMPC_S_RHO];
     auto tol = [](double b, double rel, double sgn) { return (fabs(b) > 1e300) ? b : b + sgn * rel * (1.0 + fabs(b)); };
     for (int a = 0; a < nx; a++) {
-        const double lo = sys[o.lo0 + nx + a], hi = sys[o.hi0 + nx + a];
+        const double lo = sys[o.xmin + a], hi = sys[o.xmax + a];          // the state rows of stage 1 (condensed rows nx + a)
         P.xlo[a] = lo; P.xhi[a] = hi;
         P.xlo_m[a] = tol(lo, 1e-11, -1.0); P.xlo_p[a] = tol(lo, 1e-11, 1.0); P.xhi_m[a] = tol(hi, 1e-11, -1.0); P.xhi_p[a] = tol(hi, 1e-11, 1.0);
-        P.cx[a] = rho_e / sys[o.rho + nx + a];
+        P.cx[a] = rho_e / bmpc_row_rho(lo, hi, rho);
     }
-    P.ulo = sys[o.lo0 + NX]; P.uhi = sys[o.hi0 + NX]; P.ulo_m = tol(P.ulo, 1e-9, -1.0); P.uhi_p = tol(P.uhi, 1e-9, 1.0);
-    P.dlo = sys[o.lo0 + NX + NU]; P.dhi = sys[o.hi0 + NX + NU]; P.dlo_m = tol(P.dlo, 1e-9, -1.0); P.dhi_p = tol(P.dhi, 1e-9, 1.0);
-    P.irhou = 1.0 / sys[o.rho + NX]; P.irhod = 1.0 / sys[o.rho + NX + NU];
+    // the input row and the delta-u rows (condensed rows NX and NX + NU; nu == 1)
+    P.ulo = sys[o.umin]; P.uhi = sys[o.umax]; P.ulo_m = tol(P.ulo, 1e-9, -1.0); P.uhi_p = tol(P.uhi, 1e-9, 1.0);
+    P.dlo = sys[o.Dumin]; P.dhi = sys[o.Dumax]; P.dlo_m = tol(P.dlo, 1e-9, -1.0); P.dhi_p = tol(P.dhi, 1e-9, 1.0);
+    P.irhou = 1.0 / bmpc_row_rho(P.ulo, P.uhi, rho); P.irhod = 1.0 / bmpc_row_rho(P.dlo, P.dhi, rho);
     P.Qu = sys[o.Qu]; P.QDu = sys[o.QDu]; P.quref = sys[o.Qu] * sys[o.uref]; P.rho_e = rho_e;
     const double inf = 1.0 / 0.0;
     for (int a = 0; a < nx; a++) {

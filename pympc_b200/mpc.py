@@ -369,9 +369,11 @@ class MPCController:
                     per("QxN", _dense(self.QxN), 2, self.JX_ON), per("Qu", _dense(self.Qu), 2, self.JU_ON),
                     per("QDu", _dense(self.QDu), 2, self.JDU_ON), per("xmin", args[6], 1), per("xmax", args[7], 1),
                     per("umin", args[8], 1), per("umax", args[9], 1), per("Dumin", args[10], 1), per("Dumax", args[11], 1),
-                    np.ascontiguousarray(np.broadcast_to(self.uref, (B, nu)))]
+                    per("uref", self.uref, 1)]
         self._check(L.bmpc_setup(self._h, *[ptr(a) for a in args]))
         self._Qx_d, self._QxN_d, self._Qu_d, self._QDu_d = Qx, QxN, Qu, QDu
+        # per-instance controllers: every instance's weights as sent to the device (J_CNST)
+        self._w_full = dict(zip(("Qx", "QxN", "Qu", "QDu"), args[2:6])) if self._per_instance else {}
         self._qp_static = None
         self._um1_for_J = self.uminus1_rh
         self._push(self.x0_rh, self.uminus1_rh, self.xref)
@@ -463,65 +465,136 @@ class MPCController:
         if solve:
             self.solve()
 
-    def update_system(self, Ad=None, Bd=None):
-        """Time-varying system matrices (successive linearisation, gain scheduling): replace Ad and/or Bd of the set-up controller
-        without a new setup().  The next update() is a WARM solve of the QP the reference would assemble with the new matrices
-        (working sets, ADMM state and the committed u_{-1} are kept; weights, bounds, uref and rho are unchanged).
+    # the arrays of bmpc_setup / bmpc_update_problem in argument order: (name, kind, hidden flag that zeroes it on the device)
+    _PROBLEM = (("Ad", "system", None), ("Bd", "system", None), ("Qx", "weight", "JX_ON"), ("QxN", "weight", "JX_ON"),
+                ("Qu", "weight", "JU_ON"), ("QDu", "weight", "JDU_ON"), ("xmin", "vector", None), ("xmax", "vector", None),
+                ("umin", "vector", None), ("umax", "vector", None), ("Dumin", "vector", None), ("Dumax", "vector", None),
+                ("uref", "vector", None))
+    # the constructor's messages
+    _MSG = {"Ad": "Ad should be a square matrix of dimension (nx,nx)!", "Bd": "Bd should be a matrix of dimension (nx, nu)!",
+            "Qx": "Qx should be a matrix of shape (nx, nx)!", "QxN": "QxN should be a square matrix of shape (nx, nx)!",
+            "Qu": "Qu should be a square matrix of shape (nu, nu)!", "QDu": "QDu should be a square matrix of shape (nu, nu)!",
+            "xmin": "xmin should be a vector of shape (nx,)!", "xmax": "xmax should be a vector of shape (nx,)!",
+            "umin": "umin should be a vector of shape (nu,)!", "umax": "umax should be a vector of shape (nu,)!",
+            "Dumin": "Dumin should be a vector of shape (nu,)!", "Dumax": "Dumax should be a vector of shape (nu,)!",
+            "uref": "uref should be a vector of shape (nu,)!"}
 
-        Shared controller: 2-D Ad (nx, nx) / Bd (nx, nu).  Per-instance controller: (batch, nx, nx) / (batch, nx, nu), or 2-D to give
-        every instance the same model.  Dense arrays or scipy.sparse.  The reference-form attributes (Ad, Bd, P, A, ...) follow.
-        Assigning ``K.Ad`` directly keeps the reference's meaning: no effect until setup()."""
-        Ad, Bd = self._system_arg(Ad, "Ad", (self.nx, self.nx), "Ad should be a square matrix of dimension (nx,nx)!"), \
-            self._system_arg(Bd, "Bd", (self.nx, self.nu), "Bd should be a matrix of dimension (nx, nu)!")
+    def _problem_shape(self, name):
+        nx, nu = self.nx, self.nu
+        return {"Ad": (nx, nx), "Bd": (nx, nu), "Qx": (nx, nx), "QxN": (nx, nx), "Qu": (nu, nu), "QDu": (nu, nu)}.get(
+            name, (nx,) if name in ("xmin", "xmax") else (nu,))
+
+    def update_system(self, Ad=None, Bd=None, *, Qx=None, QxN=None, Qu=None, QDu=None, xmin=None, xmax=None, umin=None, umax=None,
+                      Dumin=None, Dumax=None, uref=None):
+        """Time-varying problem data (successive linearisation, gain scheduling, derated actuator limits, tightened constraints):
+        replace any of the system matrices, weights, bounds and uref of the set-up controller without a new setup().  The next
+        update() is a WARM solve of the QP the reference would assemble with the new arrays (working sets, ADMM state, the committed
+        u_{-1} and the rho the setup chose are kept; eps_feas, SOFT_ON, the horizons and the solver options stay as set up).
+
+        Shared controller: Ad (nx, nx), Bd (nx, nu), weights (n, n), bounds and uref vectors (n,) as the constructor takes them.
+        Per-instance controller: the same, or with a leading batch dimension — (batch, n, n) matrices, (batch, n) vectors — for one
+        set per instance.  Matrices dense or scipy.sparse.  None keeps an array.  JX_ON / JU_ON / JDU_ON zero the weights sent to
+        the device as in setup().  The reference-form attributes (Ad, ..., uref, P, q, A, l, u, J_CNST) and u_failure follow;
+        assigning ``K.xmin = ...`` directly keeps the reference's meaning: no effect until setup()."""
+        B, per = self._B, self._per_instance
+        vals = dict(Ad=Ad, Bd=Bd, Qx=Qx, QxN=QxN, Qu=Qu, QDu=QDu, xmin=xmin, xmax=xmax, umin=umin, umax=umax, Dumin=Dumin, Dumax=Dumax,
+                    uref=uref)
+        given = {name: self._problem_arg(vals[name], name) for name, _, _ in self._PROBLEM if vals[name] is not None}
         if self._h is None:
             raise BmpcError("update_system() before setup()")
-        if Ad is None and Bd is None:
+        if not given:
             return
-        B = self._B
-        full = (lambda M: None if M is None else np.ascontiguousarray(np.broadcast_to(M, (B,) + M.shape[-2:]))) if self._per_instance \
-            else (lambda M: M)
-        a, b = full(Ad), full(Bd)
-        rc = self._L.bmpc_update_system(self._h, ptr(a), ptr(b), 0)
-        # the handle holds the new matrices even when the check fails (then solve() raises until a valid update): so do the attributes
-        for name, M in (("Ad", Ad), ("Bd", Bd)):
-            if M is None:
+        sent = {}
+        for name, kind, flag in self._PROBLEM:
+            if name not in given:
                 continue
-            if self._per_instance:
+            M = given[name]
+            if flag is not None and not getattr(self, flag):
+                M = np.zeros(M.shape)
+            sent[name] = np.ascontiguousarray(np.broadcast_to(M, (B,) + self._problem_shape(name))) if per else M
+        args = [ptr(sent[name]) if name in sent else None for name, _, _ in self._PROBLEM]
+        if set(given) <= {"Ad", "Bd"}:
+            rc = self._L.bmpc_update_system(self._h, args[0], args[1], 0)
+        else:
+            rc = self._L.bmpc_update_problem(self._h, *args, 0)
+        # the handle holds the new arrays even when the check fails (then solve() raises until a valid update): so do the attributes
+        for name, kind, flag in self._PROBLEM:
+            if name not in given:
+                continue
+            M = given[name]
+            full = M.ndim == len(self._problem_shape(name)) + 1
+            if per:
                 self._sys_full[name] = M
-            setattr(self, name, M[0] if M.ndim == 3 else M)
+            if kind == "weight":
+                setattr(self, name, M[0] if full else (vals[name] if hasattr(vals[name], "toarray") else M))   # (sparse stays sparse, Q16)
+                setattr(self, "_" + name + "_d", sent[name][0] if per else sent[name])
+                if per:
+                    self._w_full[name] = sent[name]
+            else:
+                setattr(self, name, M[0] if full else M)
+            if name == "uref":
+                self.u_failure = M                          # what an instance that fails outputs (per instance when given so)
         self._qp_static = None
+        self._J_dirty = True
         self._check(rc)
 
-    def _system_arg(self, M, name, shape, msg):
-        if M is None:
-            return None
-        M = np.array(M.toarray() if hasattr(M, "toarray") else M, dtype=float)          # a copy: the caller may reuse its buffer
-        if M.ndim == 3 and not self._per_instance:
+    def _problem_arg(self, val, name):
+        """validated copy (the caller may reuse its buffer) of one array of update_system: the constructor's acceptance rule and
+        message, plus a leading batch dimension on per-instance controllers"""
+        shape, B = self._problem_shape(name), self._B
+        M = np.array(val.toarray() if hasattr(val, "toarray") else val, dtype=float)
+        # a leading batch dimension: 3-D matrices; (batch, n) vectors (a (1, n) array is a vector in the reference's sense)
+        batched = M.ndim == 3 if len(shape) == 2 else (M.ndim == 2 and M.shape == (B, shape[0]) and B > 1)
+        if batched and not self._per_instance:
             raise ValueError(f"per-instance {name} of shape (batch, ...) needs a controller set up with per-instance systems "
                              "(Ad of shape (batch, nx, nx) at construction)")
-        if M.shape not in (shape, (self._B,) + shape):
-            raise ValueError(msg)
-        return M
+        if len(shape) == 2:
+            if M.shape not in (shape, (B,) + shape):
+                raise ValueError(self._MSG[name])
+            return M
+        if batched and M.shape == (B,) + shape:
+            return M
+        if __is_vector__(M) and M.size == shape[0]:
+            return M.ravel()
+        raise ValueError(self._MSG[name])
 
-    def update_system_from_device(self, Ad_ptr=None, Bd_ptr=None):
-        """update_system() with the matrices already on this controller's device (raw pointers, or contiguous float64 torch tensors),
-        e.g. a batch of linearisations computed by torch: no host round trip.  Layout as for update_system — per-instance
-        controllers (batch, nx, nx) / (batch, nx, nu), shared ones (nx, nx) / (nx, nu).  The library reads them in stream order on the
-        controller's stream: whatever wrote them must be ordered before (same stream, or synchronised); keep them unchanged until
-        the next solve has been retired.  The host-side attributes (Ad, Bd, P, A) keep describing the last host-side system."""
+    def update_system_from_device(self, Ad_ptr=None, Bd_ptr=None, *, Qx=None, QxN=None, Qu=None, QDu=None, xmin=None, xmax=None,
+                                  umin=None, umax=None, Dumin=None, Dumax=None, uref=None):
+        """update_system() with the arrays already on this controller's device (raw pointers, or contiguous float64 torch tensors),
+        e.g. a batch of linearisations or of derated limits computed by torch: no host round trip.  Per-instance controllers take
+        (batch, ...) arrays — (batch, nx, nx), (batch, nx, nu), (batch, n, n) weights, (batch, n) bounds and uref —, shared ones the
+        unbatched shapes.  The library reads them in stream order on the controller's stream: whatever wrote them must be ordered
+        before (same stream, or synchronised); keep them unchanged until the next solve has been retired.  New weights are condensed
+        and checked at once (their definiteness is not known on the host).  With JX_ON / JU_ON / JDU_ON off the weights sent are
+        zeros, as in setup().  The host-side attributes (Ad, ..., uref, P, q, A, l, u, J_CNST, u_failure) keep describing the last
+        host-side arrays."""
         if self._h is None:
             raise BmpcError("update_system_from_device() before setup()")
         n = self._B if self._per_instance else 1
-        def dev_ptr(M, shape, name):
+        vals = dict(Ad=Ad_ptr, Bd=Bd_ptr, Qx=Qx, QxN=QxN, Qu=Qu, QDu=QDu, xmin=xmin, xmax=xmax, umin=umin, umax=umax, Dumin=Dumin,
+                    Dumax=Dumax, uref=uref)
+
+        def dev_ptr(M, name, flag):
             if M is None or isinstance(M, int):
                 return M
+            shape = self._problem_shape(name)
             ok = ((n,) + shape,) if n > 1 else (shape, (1,) + shape)
             if tuple(M.shape) not in ok or not M.is_contiguous() or str(M.dtype) != "torch.float64" or not M.is_cuda \
                     or M.device.index != self.device:
                 raise ValueError(f"{name} must be a contiguous float64 CUDA tensor of shape {ok[0]}")
+            if flag is not None and not getattr(self, flag):
+                # the weight is off: zeros go to the device (a buffer the controller keeps, so it outlives the stream-ordered read)
+                zeros = self.__dict__.setdefault("_dev_zeros", {})
+                if name not in zeros:
+                    import torch
+                    zeros[name] = torch.zeros(ok[0], dtype=torch.float64, device=M.device)
+                return zeros[name].data_ptr()
             return M.data_ptr()
-        a = dev_ptr(Ad_ptr, (self.nx, self.nx), "Ad"); b = dev_ptr(Bd_ptr, (self.nx, self.nu), "Bd")
-        self._check(self._L.bmpc_update_system(self._h, a, b, 1))
+        args = [dev_ptr(vals[name], name, flag) for name, _, flag in self._PROBLEM]
+        if all(a is None for a in args[2:]):
+            self._check(self._L.bmpc_update_system(self._h, args[0], args[1], 1))
+        else:
+            self._check(self._L.bmpc_update_problem(self._h, *args, 1))
 
     def solve(self):
         """Solve the QP batch.  mpc.py:366-375."""
@@ -656,24 +729,33 @@ class MPCController:
         self._J_dirty = False
 
     def _compute_J_CNST(self):
-        """Constant of the cost exactly as the reference accumulates it (mpc.py:412-442; quirk Q7)."""
-        B, Np = self._B, self.Np
+        """Constant of the cost exactly as the reference accumulates it (mpc.py:412-442; quirk Q7).  Per-instance controllers: each
+        instance with its own weights and uref."""
+        B, Np, nu = self._B, self.Np, self.nu
         J = np.zeros(B)
-        uref = self.uref
-        um1 = np.broadcast_to(np.asarray(self._um1_for_J, dtype=float).reshape(-1, self.nu), (B, self.nu))
+        um1 = np.broadcast_to(np.asarray(self._um1_for_J, dtype=float).reshape(-1, nu), (B, nu))
+        if self._per_instance:
+            W = self._w_full
+            Qx, QxN, Qu, QDu = W["Qx"], W["QxN"], W["Qu"], W["QDu"]
+            uref = self._sys_full.get("uref")
+            uref = np.broadcast_to(np.asarray(self.uref if uref is None else uref, dtype=float).reshape(-1, nu), (B, nu))
+            quad = lambda sub, a, Q, b: np.einsum(sub.replace("ij", "bij"), a, Q, b)
+        else:
+            Qx, QxN, Qu, QDu = self._Qx_d, self._QxN_d, self._Qu_d, self._QDu_d
+            uref = self.uref
+            quad = np.einsum
         if self.JX_ON and self.COMPUTE_J_CNST:
             arr, rows = self._xref_device_layout(self.xref)
             if rows == 1:
                 xr = np.asarray(arr)
-                J += 0.5 * Np * np.einsum('bi,ij,bj->b', xr, self._QxN_d, xr) + 0.5 * np.einsum('bi,ij,bj->b', xr, self._QxN_d, xr)
+                J += 0.5 * Np * quad('bi,ij,bj->b', xr, QxN, xr) + 0.5 * quad('bi,ij,bj->b', xr, QxN, xr)
             else:
                 xr = np.asarray(arr).reshape(B, Np + 1, self.nx)
-                J += 0.5 * np.einsum('bki,ij,bkj->b', xr[:, :Np], self._Qx_d, xr[:, :Np]) + \
-                    0.5 * np.einsum('bi,ij,bj->b', xr[:, Np], self._QxN_d, xr[:, Np])
+                J += 0.5 * quad('bki,ij,bkj->b', xr[:, :Np], Qx, xr[:, :Np]) + 0.5 * quad('bi,ij,bj->b', xr[:, Np], QxN, xr[:, Np])
         if self.JU_ON:
-            J += 0.5 * Np * (uref @ (self._Qu_d @ uref))
+            J += 0.5 * Np * (quad('bi,ij,bj->b', uref, Qu, uref) if self._per_instance else uref @ (Qu @ uref))
         if self.JDU_ON:
-            J += 0.5 * np.einsum('bi,ij,bj->b', um1, self._QDu_d, um1)
+            J += 0.5 * quad('bi,ij,bj->b', um1, QDu, um1)
         self._J_CNST = J if self.batch is not None else float(J[0])
 
     # ---- reference-form QP attributes (mpc.py:597-606), built lazily on the host for instance 0 ----
