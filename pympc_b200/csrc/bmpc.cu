@@ -21,6 +21,7 @@
 #include "bmpc_rounds.cuh"
 #include "bmpc_tpi.cuh"
 #include "bmpc_tile.cuh"
+#include "bmpc_launch.cuh"
 #include "bmpc_tpm.cuh"
 #include "bmpc_dare.cuh"
 
@@ -168,11 +169,7 @@ __global__ void k_gather_arrive(long long* mine, BmpcPeerFlags P, int n_peer, in
     __threadfence_system();
 }
 
-// smem (doubles) per instance for the two kernels — keep in sync with the carve-up below
-__host__ __device__ static inline size_t admm_smem_doubles(const BmpcDims& d) { return 4 * (size_t)d.NU + d.NX + 2 * (size_t)d.mc + d.nu + 4 + 4; }
-__host__ __device__ static inline size_t polish_smem_doubles(const BmpcDims& d, int rmax) {
-    return 3 * (size_t)d.NU + d.NX + 4 * (size_t)d.mc + (size_t)rmax * (rmax + 1) / 2 + rmax + d.nu + 2 + (d.mc + rmax + 3) / 2;
-}
+// smem (doubles) per instance of the two kernels: bmpc_admm_smem_doubles, bmpc_polish_smem_doubles (bmpc_launch.cuh)
 
 __global__ void k_condense(BmpcDims d, BmpcSysOff o, double* sys, double rho, double sigma, double alpha, double eps_feas,
                            int soft_on) {
@@ -240,7 +237,7 @@ __global__ void k_admm(BmpcDims d, BmpcSysOff o, const double* __restrict__ sys,
     if (idx >= count) return;
     const int inst = list ? list[idx] : idx;
     sys += (size_t)inst * I.sys_stride;
-    double* base = smem + (size_t)slot * admm_smem_doubles(d);
+    double* base = smem + (size_t)slot * bmpc_admm_smem_doubles(d);
     double *g = base, *cc = g + d.NU, *x = cc + d.NX, *v = x + d.NU, *w = v + d.mc, *xt = w + d.mc, *r = xt + d.NU,
            *um1 = r + d.NU, *res = um1 + d.nu + (d.nu & 1);
     auto run = [&](auto& t) {
@@ -350,7 +347,7 @@ __global__ void k_polish(BmpcDims d, BmpcSysOff o, const double* __restrict__ sy
     if (idx >= count) return;
     const int inst = list ? list[idx] : idx;
     sys += (size_t)inst * I.sys_stride;
-    double* base = smem + (size_t)slot * polish_smem_doubles(d, rmax);
+    double* base = smem + (size_t)slot * bmpc_polish_smem_doubles(d, rmax);
     double *g = base, *cc = g + d.NU, *v = cc + d.NX, *W0 = v + d.mc, *zz = W0 + d.mc, *murow = zz + d.mc,
            *S = murow + d.mc, *tt = S + (size_t)rmax * (rmax + 1) / 2, *U0 = tt + rmax, *U = U0 + d.NU, *um1 = U + d.NU;
     int* st = (int*)(um1 + d.nu + (d.nu & 1));
@@ -1094,6 +1091,7 @@ struct bmpc_handle {
     size_t smem_admm = 0, smem_polish = 0;
     // low-latency CTA-per-instance variant for the few stragglers of a warp-team / TPI handle
     int fb_team = 0, fb_rmax = 0; size_t fb_smem_polish = 0;
+    bool fb_overflow = false;          // the warp-team polish hands working sets beyond rmax to this CTA tier in the same round
     int rmax_small = 0; size_t smem_polish_small = 0; int32_t* ovf = nullptr;   // small-capacity polish tier (CTA teams) + its overflow list
     int sm_count = 132;
     double* vprev = nullptr; int32_t* lprev = nullptr;   // snapshot of (v, level) for the infeasibility check of straggler rounds
@@ -1305,62 +1303,28 @@ static int configure_launch(bmpc_handle* h) {
     int dev = h->cfg.device, max_optin = 0;
     cudaDeviceGetAttribute(&max_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
     cudaDeviceGetAttribute(&h->sm_count, cudaDevAttrMultiProcessorCount, dev);
-    size_t budget = (size_t)max_optin - 1024;
-    int team = h->cfg.team_threads;
-    if (team <= 0) team = (d.mc <= 192 && d.NU <= 64) ? 32 : 256;
-    if (team != 32) { team = ((team + 31) / 32) * 32; if (team > 1024) team = 1024; }
-    h->team = team;
-    int rmax = h->cfg.rmax > 0 ? h->cfg.rmax : (team == 32 ? 64 : 224);     // S is packed: r(r+1)/2 doubles
-    if (rmax > d.mc) rmax = d.mc;
-    // shrink rmax until one instance fits
-    while (rmax > 8 && polish_smem_doubles(d, rmax) * 8 > budget) rmax -= 8;
-    if (polish_smem_doubles(d, rmax) * 8 > budget || admm_smem_doubles(d) * 8 > budget) {
-        h->err = "problem too large for the shared-memory resident kernels"; return BMPC_ERR_ARG;
-    }
-    h->rmax = rmax;
-    auto setup_tiles = [&]() -> int {
-        h->tile_T = 0;
-        if (h->cfg.team_threads == 0 && h->cfg.n_sys <= 1) {
-            for (int T : {8, 4, 2}) if (!h->tile_T && bmpc_tile_smem_doubles(d, T) * 8 <= budget) h->tile_T = T;
-            // kernels per tile size {8, 4, 2}; shapes with a compiled (nx, nu) get the unrolled instantiation
-            if (d.nx == 8 && d.nu == 4) { h->tile_fn[0] = k_admm_tile<8, 2, 8, 4>; h->tile_fn[1] = k_admm_tile<4, 2, 8, 4>; h->tile_fn[2] = k_admm_tile<2, 1, 8, 4>; }
-            else { h->tile_fn[0] = k_admm_tile<8, 2, 0, 0>; h->tile_fn[1] = k_admm_tile<4, 2, 0, 0>; h->tile_fn[2] = k_admm_tile<2, 1, 0, 0>; }
-            for (int k = 0; k < 3; k++) {
-                const int T = 8 >> k;
-                if (h->tile_T >= T) BMPC_CUDA(cudaFuncSetAttribute((const void*)h->tile_fn[k], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(bmpc_tile_smem_doubles(d, T) * 8)));
-            }
-            int th = d.NX > 2 * d.NU ? d.NX : 2 * d.NU;
-            th = ((th + 31) / 32) * 32; if (th < 128) th = 128; if (th > 512) th = 512;
-            if (h->cfg.warps_per_block > 0 && h->team != 32) th = h->cfg.warps_per_block * 32;      // tuning override
-            if (th > 512) th = 512;
-            h->tile_threads = th;
+    // team size, tiers and tile size: one decision the host emulation shares (bmpc_launch.cuh)
+    const BmpcLaunch L = bmpc_plan_launch(d, max_optin, h->cfg.team_threads, h->cfg.warps_per_block, h->cfg.rmax, h->cfg.n_sys);
+    if (!L.ok) { h->err = "problem too large for the shared-memory resident kernels"; return BMPC_ERR_ARG; }
+    h->team = L.team; h->wpb = L.wpb; h->rmax = L.rmax;
+    h->smem_admm = L.smem_admm; h->smem_polish = L.smem_polish;
+    h->fb_team = L.fb_team; h->fb_rmax = L.fb_rmax; h->fb_smem_polish = L.fb_smem_polish; h->fb_overflow = L.overflow != 0;
+    h->rmax_small = L.rmax_small; h->smem_polish_small = L.smem_polish_small;
+    h->tile_T = L.tile_T; h->tile_threads = L.tile_threads;
+    if (h->tile_T) {
+        // kernels per tile size {8, 4, 2}; shapes with a compiled (nx, nu) get the unrolled instantiation
+        if (d.nx == 8 && d.nu == 4) { h->tile_fn[0] = k_admm_tile<8, 2, 8, 4>; h->tile_fn[1] = k_admm_tile<4, 2, 8, 4>; h->tile_fn[2] = k_admm_tile<2, 1, 8, 4>; }
+        else { h->tile_fn[0] = k_admm_tile<8, 2, 0, 0>; h->tile_fn[1] = k_admm_tile<4, 2, 0, 0>; h->tile_fn[2] = k_admm_tile<2, 1, 0, 0>; }
+        for (int k = 0; k < 3; k++) {
+            const int T = 8 >> k;
+            if (h->tile_T >= T) BMPC_CUDA(cudaFuncSetAttribute((const void*)h->tile_fn[k], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(bmpc_tile_smem_doubles(d, T) * 8)));
         }
-        return BMPC_OK;
-    };
-    if (team == 32) {
-
-        int wpb = h->cfg.warps_per_block > 0 ? h->cfg.warps_per_block : 8;
-        while (wpb > 1 && (size_t)wpb * polish_smem_doubles(d, rmax) * 8 > budget) wpb--;
-        h->wpb = wpb;
-        h->smem_admm = (size_t)wpb * admm_smem_doubles(d) * 8;
-        h->smem_polish = (size_t)wpb * polish_smem_doubles(d, rmax) * 8;
+    }
+    if (h->team == 32) {
         BMPC_CUDA(cudaFuncSetAttribute(k_admm<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_admm));
         BMPC_CUDA(cudaFuncSetAttribute(k_polish<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_polish));
-        // stragglers (instances the first round did not verify) are few and latency-bound: give each a whole CTA
-        int frmax = d.mc < 128 ? d.mc : 128;
-        while (frmax > 8 && polish_smem_doubles(d, frmax) * 8 > budget) frmax -= 8;
-        if (polish_smem_doubles(d, frmax) * 8 <= budget) {
-            h->fb_team = 128; h->fb_rmax = frmax;
-            h->fb_smem_polish = polish_smem_doubles(d, frmax) * 8;
-            BMPC_CUDA(cudaFuncSetAttribute(k_polish<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->fb_smem_polish));
-        }
+        if (h->fb_team) BMPC_CUDA(cudaFuncSetAttribute(k_polish<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->fb_smem_polish));
     } else {
-        // large shapes with one shared system: the ADMM runs on tiles of T instances per CTA (bmpc_tile.cuh)
-        { int rc = setup_tiles(); if (rc) return rc; }
-        if (h->cfg.rmax == 0 && rmax > 96) { h->rmax_small = 80; h->smem_polish_small = polish_smem_doubles(d, 80) * 8; }
-        h->wpb = team / 32;
-        h->smem_admm = admm_smem_doubles(d) * 8;
-        h->smem_polish = polish_smem_doubles(d, rmax) * 8;
         BMPC_CUDA(cudaFuncSetAttribute(k_admm<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_admm));
         BMPC_CUDA(cudaFuncSetAttribute(k_polish<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_polish));
     }
@@ -1827,7 +1791,7 @@ int bmpc_update_system(bmpc_handle* h, const double* Ad, const double* Bd, int o
 }
 
 static bool use_fallback_team(const bmpc_handle* h, const int32_t* list, int count) {
-    return h->team == 32 && h->fb_team && list != nullptr && count <= 4096;
+    return h->team == 32 && h->fb_team && list != nullptr && count <= BMPC_FB_MAX_LIST;
 }
 
 static void launch_admm(bmpc_handle* h, const int32_t* list, int count, int niter, int do_prep) {
@@ -1835,7 +1799,7 @@ static void launch_admm(bmpc_handle* h, const int32_t* list, int count, int nite
     if (use_fallback_team(h, list, count)) {
         // stragglers of a warp-team / fast-path handle: one warp per CTA (the lanes-own-rows ADMM has the shortest
         // dependent chain per iteration for these small shapes: measured 5 % on the random-instance bench vs a 128-thread CTA)
-        k_admm<true><<<count, 32, admm_smem_doubles(h->d) * 8, h->stream>>>(h->d, h->o, h->sys, h->I, list, count, niter, do_prep, cold, h->xref_mode, h->cfg.polish ? 1 : 0);
+        k_admm<true><<<count, 32, bmpc_admm_smem_doubles(h->d) * 8, h->stream>>>(h->d, h->o, h->sys, h->I, list, count, niter, do_prep, cold, h->xref_mode, h->cfg.polish ? 1 : 0);
     } else if (h->team == 32 && h->tile_T == 0) {
         int grid = (count + h->wpb - 1) / h->wpb;
         k_admm<true><<<grid, h->wpb * 32, h->smem_admm, h->stream>>>(h->d, h->o, h->sys, h->I, list, count, niter, do_prep, cold, h->xref_mode, h->cfg.polish ? 1 : 0);
@@ -1856,8 +1820,14 @@ static void launch_polish(bmpc_handle* h, const int32_t* list, int count, int st
     if (use_fallback_team(h, list, count)) {
         k_polish<false><<<count, h->fb_team, h->fb_smem_polish, h->stream>>>(h->d, h->o, h->sys, h->I, list, count, h->fb_rmax, steps, next_list, next_count, h->I.u0, nullptr, nullptr, h->cfg.candidate_warm);
     } else if (h->team == 32) {
+        // working sets beyond the warp tier go to the CTA tier right after (count read on the device): whether an instance can be
+        // verified must not depend on how many instances are open
         int grid = (count + h->wpb - 1) / h->wpb;
-        k_polish<true><<<grid, h->wpb * 32, h->smem_polish, h->stream>>>(h->d, h->o, h->sys, h->I, list, count, h->rmax, steps, next_list, next_count, h->I.u0, nullptr, nullptr, h->cfg.candidate_warm);
+        k_polish<true><<<grid, h->wpb * 32, h->smem_polish, h->stream>>>(h->d, h->o, h->sys, h->I, list, count, h->rmax, steps, next_list, next_count, h->I.u0, nullptr, h->fb_overflow ? h->ovf : nullptr, h->cfg.candidate_warm);
+        if (h->fb_overflow) {
+            k_polish<false><<<count, h->fb_team, h->fb_smem_polish, h->stream>>>(h->d, h->o, h->sys, h->I, h->ovf, count, h->fb_rmax, steps, next_list, next_count, h->I.u0, next_count + 2, nullptr, h->cfg.candidate_warm);
+            h->stats.launches++;
+        }
     } else if (h->rmax_small > 0) {
         // two capacity tiers: the small one keeps several CTAs resident per SM (the polish is latency-bound); working
         // sets that outgrow it are listed and redone by the full-capacity launch right after (count read on the device)

@@ -9,11 +9,12 @@ Closed loops use the linear plant x+ = Ad x + Bd u (README.md:59-77 pattern).
     python tests/golden/make_golden.py reference    # only ref_assembly.npz and ref_on_port.npz
     python tests/golden/make_golden.py shapes       # only shapes.npz (single-input shapes at the edges of the fast path)
     python tests/golden/make_golden.py mimo_shapes  # only mimo_shapes.npz (shapes at the edges of the multi-input fast path)
+    python tests/golden/make_golden.py team_shapes  # only team_shapes.npz (team kernels: shape edges and polish capacity)
 """
 import os
 import sys
 
-if sys.argv[1:] in (["shapes"], ["mimo_shapes"]):
+if sys.argv[1:] in (["shapes"], ["mimo_shapes"], ["team_shapes"]):
     # one process per shape: single-threaded BLAS keeps them from competing and the results reproducible
     for _v in ("OPENBLAS_NUM_THREADS", "OMP_NUM_THREADS", "MKL_NUM_THREADS"):
         os.environ.setdefault(_v, "1")
@@ -312,12 +313,94 @@ def mimo_shapes():
                         pattern=np.array([s[:4] for s in MIMO_SHAPES if "pattern" in s[5]][0]), **out)
 
 
+# Team / tile kernels (k_admm, k_admm_tile, the Schur-form k_polish) at the edges of their shape domain and of the polish's
+# working-set capacity (tests/test_gpu_team_shapes.py, tests/test_team_capacity_cpu.py): (name, nx, nu, Np, Nc, scales, options).
+# Instance b starts at scales[b] times a random point of the state box: the further outside the soft box, the more soft rows are
+# violated at the optimum and the larger the polish's working set.  Options: "hard" hard state rows (SOFT_ON = False; the states
+# start inside the box), "ride" (hard) a reference beyond one state's bound, so that the state rides that bound over many stages.
+TEAM_SHAPES = [
+    ("warp_cap", 7, 1, 20, 20, (1.0, 1.4, 1.8, 2.2, 2.6, 3.0, 3.4, 4.0), ()),      # mc = 188: warp team, tiers 64 and 188
+    ("cta_cap", 5, 2, 25, 25, (1.0, 2.0, 3.0, 4.5, 6.0, 8.0, 10.0, 5.0), ()),        # mc = 232: CTA team / tile, tiers 80 and 232
+    ("mc192", 9, 1, 18, 10, (1.0, 1.5, 2.0, 3.0), ()),                             # mc = 192: the largest warp-team shape
+    ("mc193", 8, 1, 19, 16, (1.0, 1.5, 2.0, 3.0), ()),                             # mc = 193: CTA team
+    ("nu64", 1, 2, 32, 32, (1.0, 3.0, 6.0, 10.0), ()),                              # NU = 64: warp team
+    ("nu65", 1, 5, 13, 13, (1.0, 3.0, 6.0, 10.0), ()),                              # NU = 65: CTA team
+    ("tiny", 1, 1, 2, 2, (0.5, 1.5, 3.0, 6.0), ()),                                # Np = 2, nx = 1
+    ("nc1", 2, 3, 5, 1, (0.5, 1.5, 3.0, 6.0), ()),                                 # Nc = 1 with nu = 3 > nx
+    ("warp_hard", 7, 1, 20, 20, (0.05, 0.1, 0.2, 0.3), ("hard", "ride")),          # hard state rows on the warp team
+    ("cta_hard", 5, 2, 25, 25, (0.05, 0.1, 0.2, 0.3), ("hard", "ride")),           # hard state rows on the CTA team / tile
+]
+TEAM_STEPS = 4
+
+
+def working_set_size(K, z, y, tol=1e-7):
+    """size of the polish's working set at the optimum (z, y) of the reference-assembled QP: soft rows outside their box (non-zero
+    slack) plus inequality rows without slack at a bound with a non-zero multiplier"""
+    A = K.A.toarray(); NX, NU = (K.Np + 1) * K.nx, K.Nc * K.nu
+    nz = A.shape[1] - NX - NU                                    # slack columns (SOFT_ON)
+    soft_rows = np.abs(A[:, NX + NU:]).sum(axis=1) > 0 if nz else np.zeros(A.shape[0], bool)
+    ineq = (K.u - K.l) > 1e-12
+    slack = np.abs(z[NX + NU:]) > tol * (1.0 + np.abs(z[:NX]).max()) if nz else np.zeros(0, bool)
+    hard = ineq & ~soft_rows & (np.abs(y) > tol * (1.0 + np.abs(y).max()))
+    return int(slack.sum() + hard.sum())
+
+
+def team_shape_case(spec):
+    name, nx, nu, Np, Nc, scales, opts = spec
+    rng = np.random.default_rng([2028, nx, nu, Np, Nc, len(opts)])
+    c = random_system(rng, nx, nu, Np, Nc)
+    c["uref"] = np.zeros(nu)
+    N = len(scales)
+    P0 = rng.uniform(c["xmin"], c["xmax"], (N, nx))
+    X0 = np.array(scales)[:, None] * np.where(rng.uniform(size=(N, nx)) < 0.5, c["xmin"], c["xmax"]) if "hard" not in opts else \
+        np.array(scales)[:, None] * P0
+    if "hard" not in opts:
+        X0 = 0.5 * (X0 + np.array(scales)[:, None] * P0)
+    Xref = 0.5 * rng.standard_normal((N, nx))
+    if "ride" in opts:
+        c["Qx"][0, 0] = c["QxN"][0, 0] = 20.0                      # a heavy weight on a reference beyond the hard bound: state 0
+        Xref[:, 0] = 3.0 * c["xmax"][0]                            # rides its bound over the horizon
+    NX, NU = (Np + 1) * nx, Nc * nu
+    X = np.zeros((TEAM_STEPS, N, nx)); U = np.zeros((TEAM_STEPS, N, nu)); useq = np.zeros((TEAM_STEPS, N, NU))
+    WS = np.zeros((TEAM_STEPS, N), np.int64)
+    for b in range(N):
+        K = MPC(**dict(c, x0=X0[b], xref=Xref[b], uminus1=np.zeros(nu)))
+        if "hard" in opts:
+            K.SOFT_ON = False
+        K.setup(solve=False)
+        x = X0[b].copy(); um1 = np.zeros(nu); warm = None
+        for t in range(TEAM_STEPS):
+            K.update(x, um1, solve=False)
+            z, y, r = certified(K, warm); warm = (z, y)
+            X[t, b] = x; useq[t, b] = z[NX:NX + NU]; U[t, b] = z[NX:NX + nu]; WS[t, b] = working_set_size(K, z, y)
+            um1 = z[NX:NX + nu].copy(); x = c["Ad"] @ x + c["Bd"] @ um1
+    tag = name + "_"
+    out = {tag + k: np.asarray(v, float) for k, v in c.items() if k not in ("Np", "Nc")}
+    out.update({tag + "X": X, tag + "U": U, tag + "useq": useq, tag + "Xref": Xref, tag + "ws": WS,
+                tag + "shape": np.array([nx, nu, Np, Nc]), tag + "hard": np.array("hard" in opts)})
+    print("team_shapes", name, (nx, nu, Np, Nc), "working sets", WS.tolist(), flush=True)
+    return out
+
+
+def team_shapes():
+    from multiprocessing import Pool
+    with Pool(min(len(TEAM_SHAPES), os.cpu_count() or 1)) as pool:
+        parts = pool.map(team_shape_case, sorted(TEAM_SHAPES, key=lambda s: -((s[3] + 1) * s[1] + s[4] * s[2]) ** 2 * len(s[5])))
+    out = {}
+    for p in parts:
+        out.update(p)
+    np.savez_compressed(os.path.join(OUT, "team_shapes.npz"), names=np.array([s[0] for s in TEAM_SHAPES]), steps=TEAM_STEPS, **out)
+
+
 if __name__ == "__main__":
     if sys.argv[1:] == ["shapes"]:
         shapes()
         sys.exit(0)
     if sys.argv[1:] == ["mimo_shapes"]:
         mimo_shapes()
+        sys.exit(0)
+    if sys.argv[1:] == ["team_shapes"]:
+        team_shapes()
         sys.exit(0)
     if sys.argv[1:] == ["reference"]:        # only the records of the reference's solver inputs (tests/test_oracle.py)
         reference_assembly(); reference_on_port()
@@ -331,3 +414,4 @@ if __name__ == "__main__":
     reference_assembly(); reference_on_port()
     shapes()
     mimo_shapes()
+    team_shapes()

@@ -15,7 +15,7 @@ _NAMES = ["Ad", "Bd", "Qx", "QxN", "Qu", "QDu", "xmin", "xmax", "umin", "umax", 
 def build():
     src = os.path.join(_HERE, "hostemu.cpp")
     csrc = os.path.join(_HERE, "..", "..", "pympc_b200", "csrc")
-    deps = [src] + [os.path.join(csrc, f) for f in ("bmpc_core.cuh", "bmpc_rounds.cuh", "bmpc_tpi.cuh", "bmpc_tile.cuh", "bmpc_tpm.cuh")]
+    deps = [src] + [os.path.join(csrc, f) for f in ("bmpc_core.cuh", "bmpc_rounds.cuh", "bmpc_launch.cuh", "bmpc_tpi.cuh", "bmpc_tile.cuh", "bmpc_tpm.cuh")]
     os.makedirs(os.path.dirname(_SO), exist_ok=True)
     if (not os.path.exists(_SO)) or os.path.getmtime(_SO) < max(os.path.getmtime(p) for p in deps):
         subprocess.check_call(["g++", "-O2", "-shared", "-fPIC", "-Wno-unknown-pragmas", "-x", "c++", src, "-o", _SO])
@@ -57,15 +57,18 @@ class EmuSystem:
         n = int(np.prod(shape))
         return self.sys[self.off[name]:self.off[name] + n].reshape(shape).copy()
 
-    def solve(self, x0, um1, xref, first_iters=10, max_iter=4000, pdas_steps=10, rmax=64, eps_abs=1e-3, eps_rel=1e-3):
+    def solve(self, x0, um1, xref, first_iters=10, max_iter=4000, pdas_steps=10, rmax=64, eps_abs=1e-3, eps_rel=1e-3, tiers=None):
+        """rounds of ADMM + Schur polish.  The polish capacity is rmax, or tiers = (first round, straggler rounds): the capacities of
+        the device's polish tiers in each (launch_tiers), smallest first."""
         x0 = np.ascontiguousarray(x0, float); um1 = np.ascontiguousarray(um1, float); xref = np.ascontiguousarray(xref, float)
         mode = 0 if xref.ndim == 1 else 1
+        t0, t1 = (np.ascontiguousarray(t, np.int32) for t in (tiers or ((rmax,), (rmax,))))
         U = np.zeros(self.NU); it = ctypes.c_int(); ps = ctypes.c_int(); res = np.zeros(4)
         f = self.L.emu_solve
         f.argtypes = [ctypes.c_int] * 4 + [ctypes.c_void_p] * 4 + [ctypes.c_int] * 2 + [ctypes.c_void_p] * 3 + \
-                     [ctypes.c_int] * 4 + [ctypes.c_double] * 2 + [ctypes.c_void_p] * 3
+                     [ctypes.c_int] * 3 + [ctypes.c_void_p, ctypes.c_int] * 2 + [ctypes.c_double] * 2 + [ctypes.c_void_p] * 3
         st = f(self.nx, self.nu, self.Np, self.Nc, _p(self.sys), _p(x0), _p(um1), _p(xref), mode, self.cold,
-               _p(self.x), _p(self.v), _p(U), first_iters, max_iter, pdas_steps, rmax, eps_abs, eps_rel,
+               _p(self.x), _p(self.v), _p(U), first_iters, max_iter, pdas_steps, _p(t0), len(t0), _p(t1), len(t1), eps_abs, eps_rel,
                ctypes.byref(it), ctypes.byref(ps), _p(res))
         self.cold = 0
         return U, st, it.value, ps.value, res
@@ -160,3 +163,32 @@ class EmuSystem:
         f = self.L.emu_infeasible
         f.argtypes = [ctypes.c_int] * 4 + [ctypes.c_void_p] * 4 + [ctypes.c_int] * 2 + [ctypes.c_double]
         return bool(f(self.nx, self.nu, self.Np, self.Nc, _p(self.sys), _p(x0), _p(um1), _p(xref), it0, it1, eps))
+
+
+# opt-in shared memory per block of an H100 (cudaDevAttrMaxSharedMemoryPerBlockOptin), bytes
+H100_OPTIN = 232448
+_LAUNCH_FIELDS = ("ok", "team", "wpb", "rmax", "rmax_small", "fb_team", "fb_rmax", "overflow", "tile_T", "tile_threads",
+                  "smem_admm", "smem_polish", "smem_polish_small", "fb_smem_polish")
+
+
+def plan_launch(nx, nu, Np, Nc=None, max_optin=H100_OPTIN, team_threads=0, warps_per_block=0, rmax=0, n_sys=1):
+    """the launch configuration bmpc_create chooses (bmpc_launch.cuh: bmpc_plan_launch), as a dict"""
+    L = build(); out = np.zeros(14, np.int64)
+    f = L.emu_plan_launch
+    f.restype = None
+    f.argtypes = [ctypes.c_int] * 9 + [ctypes.c_void_p]
+    f(nx, nu, Np, Nc or Np, max_optin, team_threads, warps_per_block, rmax, n_sys, _p(out))
+    return dict(zip(_LAUNCH_FIELDS, (int(v) for v in out)))
+
+
+def launch_tiers(nx, nu, Np, Nc=None, count=1, max_optin=H100_OPTIN, team_threads=0, warps_per_block=0, rmax=0, n_sys=1):
+    """(first round, straggler rounds): capacities of the polish tiers an instance passes in a batch of `count` whose straggler
+    rounds keep all of them open (bmpc_polish_tiers), smallest first"""
+    L = build(); caps = np.zeros(2, np.int32)
+    f = L.emu_polish_tiers
+    f.argtypes = [ctypes.c_int] * 11 + [ctypes.c_void_p]
+    out = []
+    for given in (0, 1):
+        n = f(nx, nu, Np, Nc or Np, max_optin, team_threads, warps_per_block, rmax, n_sys, count, given, _p(caps))
+        out.append(tuple(int(c) for c in caps[:n]))
+    return tuple(out)

@@ -9,6 +9,7 @@
 #include "../../pympc_b200/csrc/bmpc_core.cuh"
 #include "../../pympc_b200/csrc/bmpc_tpi.cuh"
 #include "../../pympc_b200/csrc/bmpc_tile.cuh"
+#include "../../pympc_b200/csrc/bmpc_launch.cuh"
 #include <stdlib.h>
 #include <stdio.h>
 #include <string.h>
@@ -32,13 +33,35 @@ void emu_condense(int nx, int nu, int Np, int Nc, double* sys, double rho, doubl
     bmpc_condense(t, d, o, sys, rho, sigma, alpha, eps_feas, soft_on);
 }
 
-// one full solve of one instance: rounds of ADMM + polish, like the host loop of the library.
+// the launch configuration bmpc_create chooses (bmpc_plan_launch): out[14] = ok, team, wpb, rmax, rmax_small, fb_team, fb_rmax,
+// overflow, tile_T, tile_threads, smem_admm, smem_polish, smem_polish_small, fb_smem_polish
+void emu_plan_launch(int nx, int nu, int Np, int Nc, int max_optin, int team_threads, int warps_per_block, int rmax, int n_sys, long long* out) {
+    const BmpcLaunch L = bmpc_plan_launch(bmpc_make_dims(nx, nu, Np, Nc), max_optin, team_threads, warps_per_block, rmax, n_sys);
+    const long long v[14] = {L.ok, L.team, L.wpb, L.rmax, L.rmax_small, L.fb_team, L.fb_rmax, L.overflow, L.tile_T, L.tile_threads,
+                             (long long)L.smem_admm, (long long)L.smem_polish, (long long)L.smem_polish_small, (long long)L.fb_smem_polish};
+    for (int k = 0; k < 14; k++) out[k] = v[k];
+}
+
+// capacities of the polish tiers of one round over `count` open instances (bmpc_polish_tiers); returns how many
+int emu_polish_tiers(int nx, int nu, int Np, int Nc, int max_optin, int team_threads, int warps_per_block, int rmax, int n_sys,
+                     int count, int list_given, int* caps) {
+    const BmpcLaunch L = bmpc_plan_launch(bmpc_make_dims(nx, nu, Np, Nc), max_optin, team_threads, warps_per_block, rmax, n_sys);
+    return L.ok ? bmpc_polish_tiers(L, count, list_given != 0, caps) : 0;
+}
+
+// one full solve of one instance: rounds of ADMM + polish, like the host loop of the library.  The polish of each round runs
+// its tiers like the device: tiers0 [n0] in the first round, tiers1 [n1] in the straggler rounds, smallest capacity first; a
+// working set beyond one tier's capacity is redone by the next.
 // x,v: warm start in/out (cold != 0 -> initialise).  Returns status (1 solved+polished, 2 solved by eps only, -2 max iter).
 int emu_solve(int nx, int nu, int Np, int Nc, const double* sys, const double* x0, const double* um1, const double* xref,
               int xref_mode, int cold, double* x, double* v, double* Uout, int first_iters, int max_iter, int pdas_steps,
-              int rmax, double eps_abs, double eps_rel, int* iters_out, int* polish_steps_out, double* res_out) {
+              const int* tiers0, int n0, const int* tiers1, int n1, double eps_abs, double eps_rel, int* iters_out,
+              int* polish_steps_out, double* res_out) {
     BmpcDims d = bmpc_make_dims(nx, nu, Np, Nc); BmpcSysOff o = bmpc_make_off(d);
     SeqTeam t;
+    int rmax = 1;
+    for (int k = 0; k < n0; k++) rmax = tiers0[k] > rmax ? tiers0[k] : rmax;
+    for (int k = 0; k < n1; k++) rmax = tiers1[k] > rmax ? tiers1[k] : rmax;
     double* buf = (double*)calloc(8 * d.mc + 8 * d.NU + d.NX + rmax * (rmax + 1) / 2 + rmax + 16, sizeof(double));
     double *g = buf, *cc = g + d.NU, *w = cc + d.NX, *xt = w + d.mc, *r = xt + d.NU, *W0 = r + d.NU, *zz = W0 + d.mc,
            *murow = zz + d.mc, *S = murow + d.mc, *tt = S + rmax * (rmax + 1) / 2, *U0 = tt + rmax, *U = U0 + d.NU, *res = U + d.NU;
@@ -54,7 +77,9 @@ int emu_solve(int nx, int nu, int Np, int Nc, const double* sys, const double* x
         bmpc_admm(t, d, o, sys, um1, g, cc, x, v, w, xt, r, pl.chunk, res, lvl);
         lvl = bmpc_adapt_level(t, d, o, sys, um1, v, res, lvl);
         total += pl.chunk;
-        int ps = bmpc_polish(t, d, o, sys, um1, g, cc, v, W0, zz, murow, st, S, tt, R, U0, U, rmax, pl.cap);
+        const int* tiers = round == 0 ? tiers0 : tiers1; const int ntiers = round == 0 ? n0 : n1;
+        int ps = -1;
+        for (int k = 0; k < ntiers && ps == -1; k++) ps = bmpc_polish(t, d, o, sys, um1, g, cc, v, W0, zz, murow, st, S, tt, R, U0, U, tiers[k], pl.cap);
         if (getenv("EMU_TRACE")) printf("TRACE %d %.3e %.3e %d\n", total, res[0] / fmax(res[2], 1e-12), res[1] / fmax(res[3], 1e-12), ps);
         if (ps > 0) {
             psteps += ps; status = 1;

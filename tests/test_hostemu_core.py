@@ -5,7 +5,7 @@ import numpy as np
 import pytest
 
 from conftest import golden
-from emu import EmuSystem
+from emu import EmuSystem, launch_tiers
 from oracle.qp_assembly import QPData
 from pympc_b200.workloads import point_mass, pendulum, mimo
 
@@ -303,7 +303,7 @@ def test_far_outside_failure_rate_is_the_osqp_restatements():
         c = random_system(rng, 4, 1, 20, None, 1e5)
         c["x0"] = rng.uniform(2.5 * c["xmin"], 2.5 * c["xmax"]); c["xref"] = 0.5 * rng.standard_normal(4); c["uminus1"] = np.zeros(1)
         E = EmuSystem(c)
-        U, st, it, ps, res = E.solve(c["x0"], c["uminus1"], c["xref"], first_iters=50, rmax=min(E.mc, 128))
+        U, st, it, ps, res = E.solve(c["x0"], c["uminus1"], c["xref"], first_iters=50, tiers=launch_tiers(4, 1, 20, count=1))
         Q = QPData(**c)
         S = osqp_port.OSQP(); S.setup(sp.csc_matrix(Q.P), Q.q, sp.csc_matrix(Q.A), Q.l, Q.u, warm_start=True, verbose=False, eps_abs=1e-3, eps_rel=1e-3)
         ref_fail += S.solve().info.status_val != 1
