@@ -92,7 +92,9 @@ void bmpc_destroy(bmpc_handle* h);
 const char* bmpc_last_error(const bmpc_handle* h);   /* h may be NULL: error of the last failed bmpc_create */
 
 /* replaces _compute_QP_matrices_ + OSQP.setup (mpc.py:254-269, 456-615): condense + factor on device (K1).
- * All pointers are HOST pointers; each array carries a leading n_sys dimension (n_sys = 1: one shared system). */
+ * All pointers are HOST pointers; each array carries a leading n_sys dimension (n_sys = 1: one shared system).
+ * BMPC_ERR_NOT_PD on a handle set up before: the handle holds the new arrays and bmpc_solve returns BMPC_ERR_STATE until a
+ * successful bmpc_setup or update. */
 int bmpc_setup(bmpc_handle* h, const double* Ad, const double* Bd, const double* Qx, const double* QxN,
                const double* Qu, const double* QDu, const double* xmin, const double* xmax, const double* umin,
                const double* umax, const double* Dumin, const double* Dumax, const double* uref);

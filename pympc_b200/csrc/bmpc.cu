@@ -13,6 +13,7 @@
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
+#include <array>
 #include <string>
 #include <vector>
 
@@ -1254,6 +1255,13 @@ static const TpmEntry g_tpm_table[] = {
 #undef BMPC_TPM_SPARSE_SHAPE
 static const int g_tpm_count = (int)(sizeof(g_tpm_table) / sizeof(g_tpm_table[0]));
 
+// index of the first entry at or after `from` of a compiled table (g_tpi_table, g_tpm_table) with d's (nx, nu, Np, Nc); -1: none
+template <class E>
+static int find_shape(const E* table, int count, const BmpcDims& d, int from = 0) {
+    for (int k = from; k < count; k++)
+        if (table[k].nx == d.nx && table[k].nu == d.nu && table[k].Np == d.Np && table[k].Nc == d.Nc) return k;
+    return -1;
+}
 
 extern "C" {
 
@@ -1268,17 +1276,11 @@ void bmpc_default_config(bmpc_config* c) {
 }
 
 int bmpc_has_fast_path(int nx, int nu, int Np, int Nc) {
-    if (Nc <= 0) Nc = Np;
-    for (int k = 0; k < g_tpi_count; k++)
-        if (g_tpi_table[k].nx == nx && g_tpi_table[k].nu == nu && g_tpi_table[k].Np == Np && g_tpi_table[k].Nc == Nc) return 1;
-    return 0;
+    return find_shape(g_tpi_table, g_tpi_count, bmpc_make_dims(nx, nu, Np, Nc <= 0 ? Np : Nc)) >= 0;
 }
 
 int bmpc_has_multi_input_fast_path(int nx, int nu, int Np, int Nc) {
-    if (Nc <= 0) Nc = Np;
-    for (int k = 0; k < g_tpm_count; k++)
-        if (g_tpm_table[k].nx == nx && g_tpm_table[k].nu == nu && g_tpm_table[k].Np == Np && g_tpm_table[k].Nc == Nc) return 1;
-    return 0;
+    return find_shape(g_tpm_table, g_tpm_count, bmpc_make_dims(nx, nu, Np, Nc <= 0 ? Np : Nc)) >= 0;
 }
 
 int bmpc_device_count(void) {
@@ -1489,7 +1491,15 @@ int bmpc_get_dims(const bmpc_handle* h, int32_t* dims) {
     return BMPC_OK;
 }
 
-// ---- helpers of bmpc_setup and bmpc_update_system
+// ---- helpers of bmpc_setup and bmpc_update_problem
+// the 13 input arrays of bmpc_setup / bmpc_update_problem in argument order: block offset and doubles per system
+struct BmpcInput { int off, cnt; };
+static std::array<BmpcInput, 13> problem_inputs(const BmpcDims& d, const BmpcSysOff& o) {
+    const int xx = d.nx * d.nx, uu = d.nu * d.nu;
+    return {{{o.Ad, xx}, {o.Bd, d.nx * d.nu}, {o.Qx, xx}, {o.QxN, xx}, {o.Qu, uu}, {o.QDu, uu}, {o.xmin, d.nx}, {o.xmax, d.nx},
+             {o.umin, d.nu}, {o.umax, d.nu}, {o.Dumin, d.nu}, {o.Dumax, d.nu}, {o.uref, d.nu}}};
+}
+
 // x'Qx > 0 for every x != 0: Cholesky factorisation of the symmetric part
 static bool host_pd(const double* Q, int n) {
     std::vector<double> L((size_t)n * n);
@@ -1517,10 +1527,31 @@ static bool host_psd(const double* Q, int n) {
     return diag ? nonneg : host_pd(Q, n);
 }
 // H = B'P_X B + P_U is positive definite for ANY (Ad, Bd) when P_X >= 0 and P_U > 0 (Qx, QxN, Qu, QDu >= 0 and Qu or QDu > 0: the
-// difference matrix T is positive definite); w: the weights Qx, QxN, Qu, QDu of one system, contiguous as in its block
-static bool weights_keep_h_definite(const BmpcDims& d, const double* w) {
-    const double *Qx = w, *QxN = Qx + d.nx * d.nx, *Qu = QxN + d.nx * d.nx, *QDu = Qu + d.nu * d.nu;
-    return host_psd(Qx, d.nx) && host_psd(QxN, d.nx) && host_psd(Qu, d.nu) && host_psd(QDu, d.nu) && (host_pd(Qu, d.nu) || host_pd(QDu, d.nu));
+// difference matrix T is positive definite).  Per-instance systems whose weights all do so may defer the condense (sys_lazy).
+// w: the weights Qx, QxN, Qu, QDu of n systems, each system's contiguous as in its block, system i's at w + i * stride
+static bool weights_keep_h_definite(const BmpcDims& d, const double* w, int n, size_t stride) {
+    for (int i = 0; i < n; i++, w += stride) {
+        const double *Qx = w, *QxN = Qx + d.nx * d.nx, *Qu = QxN + d.nx * d.nx, *QDu = Qu + d.nu * d.nu;
+        if (!(host_psd(Qx, d.nx) && host_psd(QxN, d.nx) && host_psd(Qu, d.nu) && host_psd(QDu, d.nu) && (host_pd(Qu, d.nu) || host_pd(QDu, d.nu))))
+            return false;
+    }
+    return true;
+}
+
+// condensed Hessians of all n_sys systems positive definite; otherwise bmpc_solve refuses until the next successful
+// bmpc_update_problem / bmpc_setup.  who: the entry point named in the message
+static int check_condensed(bmpc_handle* h, const char* who) {
+    const int ns = h->cfg.n_sys; const BmpcSysOff& o = h->o;
+    std::vector<double> errs(ns);
+    BMPC_CUDA(cudaMemcpy2DAsync(errs.data(), sizeof(double), h->sys + o.scal + BMPC_S_ERR, sizeof(double) * o.total, sizeof(double), ns,
+                                cudaMemcpyDeviceToHost, h->stream));
+    BMPC_CUDA(cudaStreamSynchronize(h->stream));
+    for (int si = 0; si < ns; si++) if (errs[si] != 0.0) {
+        h->sys_bad = true;
+        h->err = std::string(who) + ": condensed Hessian is not positive definite (the weights or (Ad, Bd) make the QP non-strictly convex in U)";
+        return BMPC_ERR_NOT_PD;
+    }
+    return BMPC_OK;
 }
 
 // multi-input fast path: the first compiled entry of the shape whose (Ad, Bd) pattern masks contain the system's (blk: system block
@@ -1535,9 +1566,8 @@ static int tpm_match(const bmpc_handle* h, const double* blk) {
         for (int i = 0; i < d.nx * d.nx; i++) if (blk[o.Ad + i] != 0.0) am |= 1ull << i;
         for (int i = 0; i < d.nx * d.nu; i++) if (blk[o.Bd + i] != 0.0) bm |= 1u << i;
     } else { am = ~0ull; bm = ~0u; }
-    for (int k = 0; k < g_tpm_count; k++)
-        if (g_tpm_table[k].nx == d.nx && g_tpm_table[k].nu == d.nu && g_tpm_table[k].Np == d.Np && g_tpm_table[k].Nc == d.Nc &&
-            (am & ~g_tpm_table[k].amask) == 0ull && (bm & ~g_tpm_table[k].bmask) == 0u) return k + 1;
+    for (int k = find_shape(g_tpm_table, g_tpm_count, d); k >= 0; k = find_shape(g_tpm_table, g_tpm_count, d, k + 1))
+        if ((am & ~g_tpm_table[k].amask) == 0ull && (bm & ~g_tpm_table[k].bmask) == 0u) return k + 1;
     return 0;
 }
 // parameter block and workspace of multi-input entry `kind` from the condensed block hs (host copy); the entry stays off when its
@@ -1560,6 +1590,25 @@ static int policy_family(const bmpc_handle* h) {
     return h->tpi_kind ? (h->tpi_view ? BMPC_FAM_TPI_VIEW : BMPC_FAM_TPI) : h->tpm_kind ? BMPC_FAM_TPM : BMPC_FAM_TEAM;
 }
 
+// what the host derives from system 0's condensed block (bmpc_setup; bmpc_update_problem on a shared system): the single-input fast
+// path's constant-bank parameters, the multi-input entry and the kernel family.  Reads the block back only when a fast path is in play
+// (the single-input one, or multi-input entries of this shape: their pattern match reads Ad, Bd).  fresh: empty multi-input records
+static int derive_from_block(bmpc_handle* h, bool fresh) {
+    const int old = h->tpm_kind;
+    const bool tpm = tpm_eligible(h) && find_shape(g_tpm_table, g_tpm_count, h->d) >= 0;
+    h->tpm_kind = 0;
+    if (h->tpi_kind || tpm) {
+        std::vector<double> hs(h->o.total);
+        BMPC_CUDA(cudaMemcpyAsync(hs.data(), h->sys, sizeof(double) * h->o.total, cudaMemcpyDeviceToHost, h->stream));
+        BMPC_CUDA(cudaStreamSynchronize(h->stream));
+        if (h->tpi_kind) g_tpi_table[h->tpi_kind - 1].fill(hs.data(), h->o, h->tpi_admm_params, h->tpi_polish_params);
+        const int tk = tpm ? tpm_match(h, hs.data()) : 0;
+        if (tk) { int rc = tpm_prepare(h, hs.data(), tk, fresh || tk != old); if (rc) return rc; }
+    }
+    h->policy.family = policy_family(h);
+    return BMPC_OK;
+}
+
 // per-instance systems after bmpc_update_system: bring the condensed blocks of the listed instances (nullptr: 0..count-1) up to date
 // before a launch that reads them; instances already fresh cost one CTA that leaves at once.  Returns 1 if it launched.
 static int condense_stale(bmpc_handle* h, const int32_t* list, int count, int32_t* ncount) {
@@ -1574,48 +1623,29 @@ int bmpc_setup(bmpc_handle* h, const double* Ad, const double* Bd, const double*
                const double* QDu, const double* xmin, const double* xmax, const double* umin, const double* umax,
                const double* Dumin, const double* Dumax, const double* uref) {
     if (!h) return BMPC_ERR_ARG;
-    if (!Ad || !Bd || !Qx || !QxN || !Qu || !QDu || !xmin || !xmax || !umin || !umax || !Dumin || !Dumax || !uref) {
-        h->err = "bmpc_setup: null pointer"; return BMPC_ERR_ARG;
-    }
+    const double* src[13] = {Ad, Bd, Qx, QxN, Qu, QDu, xmin, xmax, umin, umax, Dumin, Dumax, uref};
+    for (const double* s : src) if (!s) { h->err = "bmpc_setup: null pointer"; return BMPC_ERR_ARG; }
     BMPC_CUDA(cudaSetDevice(h->cfg.device));
     const BmpcDims& d = h->d; const BmpcSysOff& o = h->o;
     const int ns = h->cfg.n_sys;
+    const auto P = problem_inputs(d, o);
     std::vector<double> in((size_t)o.pw * ns, 0.0);
-    for (int si = 0; si < ns; si++) {
-        double* blk = in.data() + (size_t)si * o.pw;
-        auto put = [&](int off, const double* src, int cnt) { memcpy(blk + off, src + (size_t)si * cnt, sizeof(double) * cnt); };
-        put(o.Ad, Ad, d.nx * d.nx); put(o.Bd, Bd, d.nx * d.nu); put(o.Qx, Qx, d.nx * d.nx); put(o.QxN, QxN, d.nx * d.nx);
-        put(o.Qu, Qu, d.nu * d.nu); put(o.QDu, QDu, d.nu * d.nu); put(o.xmin, xmin, d.nx); put(o.xmax, xmax, d.nx);
-        put(o.umin, umin, d.nu); put(o.umax, umax, d.nu); put(o.Dumin, Dumin, d.nu); put(o.Dumax, Dumax, d.nu); put(o.uref, uref, d.nu);
-    }
+    for (int si = 0; si < ns; si++)
+        for (int f = 0; f < 13; f++) memcpy(in.data() + (size_t)si * o.pw + P[f].off, src[f] + (size_t)si * P[f].cnt, sizeof(double) * P[f].cnt);
     BMPC_CUDA(cudaMemcpy2DAsync(h->sys, sizeof(double) * o.total, in.data(), sizeof(double) * o.pw, sizeof(double) * o.pw, ns,
                                 cudaMemcpyHostToDevice, h->stream));
     k_condense<<<ns, 256, 0, h->stream>>>(d, o, h->sys, h->cfg.rho, h->cfg.sigma, h->cfg.alpha, h->cfg.eps_feas, h->cfg.soft_on);
     BMPC_CUDA(cudaGetLastError());
-    std::vector<double> errs(ns);
-    BMPC_CUDA(cudaMemcpy2DAsync(errs.data(), sizeof(double), h->sys + o.scal + BMPC_S_ERR, sizeof(double) * o.total, sizeof(double), ns,
-                                cudaMemcpyDeviceToHost, h->stream));
-    BMPC_CUDA(cudaStreamSynchronize(h->stream));
-    for (int si = 0; si < ns; si++) if (errs[si] != 0.0) {
-        h->err = "condensed Hessian is not positive definite (Qu/QDu/Qx make the QP non-strictly convex in U)";
-        return BMPC_ERR_NOT_PD;
-    }
+    // everything derived from the new arrays comes before the check: a handle refused after a failed setup still describes what its
+    // blocks hold, so a later update decides and refreshes from the same state as after a failed update
     // thread-per-instance fast path for the compiled small shapes (pendulum, point mass)
-    h->tpi_kind = 0;
     // (the Riccati polish treats state rows as the soft penalty they are by default; hard state rows -> team kernels)
-    if (h->cfg.fast_path && h->team == 32 && h->cfg.soft_on) {
-        for (int k = 0; k < g_tpi_count; k++)
-            if (g_tpi_table[k].nx == d.nx && g_tpi_table[k].nu == d.nu && g_tpi_table[k].Np == d.Np && g_tpi_table[k].Nc == d.Nc) { h->tpi_kind = k + 1; break; }
-    }
+    h->tpi_kind = h->cfg.fast_path && h->team == 32 && h->cfg.soft_on ? find_shape(g_tpi_table, g_tpi_count, d) + 1 : 0;
     if (h->tpi_kind) {
         const TpiEntry& te = g_tpi_table[h->tpi_kind - 1];
         if (te.code_stride > h->code_stride) { h->err = "fast path: working-set record larger than allocated"; return BMPC_ERR_STATE; }
-        std::vector<double> hs(o.total);
-        BMPC_CUDA(cudaMemcpyAsync(hs.data(), h->sys, sizeof(double) * o.total, cudaMemcpyDeviceToHost, h->stream));
-        BMPC_CUDA(cudaStreamSynchronize(h->stream));
         free(h->tpi_admm_params); free(h->tpi_polish_params);
         h->tpi_admm_params = malloc(te.admm_bytes); h->tpi_polish_params = malloc(te.ric_bytes);
-        te.fill(hs.data(), o, h->tpi_admm_params, h->tpi_polish_params);          // system 0 (the only one when the system is shared)
         if (te.configure()) { h->err = "fast path: shared-memory configuration failed"; return BMPC_ERR_CUDA; }
         if (h->tpi_view) { cudaFree(h->tpi_view); h->tpi_view = nullptr; }
         if (ns > 1) {
@@ -1625,29 +1655,23 @@ int bmpc_setup(bmpc_handle* h, const double* Ad, const double* Bd, const double*
             BMPC_CUDA(cudaGetLastError());
         }
     }
-    // multi-input fast path: compiled shape, one shared system, soft state rows, diagonal QDu
-    // (sparsity pattern of (Ad, Bd): an entry fits when its compile-time masks contain it)
-    h->tpm_kind = 0;
-    const int tk = tpm_eligible(h) ? tpm_match(h, in.data()) : 0;
-    if (tk) {
-        std::vector<double> hs(o.total);
-        BMPC_CUDA(cudaMemcpyAsync(hs.data(), h->sys, sizeof(double) * o.total, cudaMemcpyDeviceToHost, h->stream));
-        BMPC_CUDA(cudaStreamSynchronize(h->stream));
-        int rc = tpm_prepare(h, hs.data(), tk, true);
-        if (rc) return rc;
-    }
+    // the fast paths' parameters and the kernel family; multi-input fast path: compiled shape, one shared system, soft state rows,
+    // diagonal QDu (sparsity pattern of (Ad, Bd): an entry fits when its compile-time masks contain it)
+    int rc = derive_from_block(h, true);
+    if (rc) return rc;
     const bmpc_config& c = h->cfg;
-    h->policy = bmpc_make_policy(policy_family(h), c.polish, c.first_iters, c.cold_iters, c.max_iter, c.pdas_steps, c.shift_warm);
+    h->policy = bmpc_make_policy(h->policy.family, c.polish, c.first_iters, c.cold_iters, c.max_iter, c.pdas_steps, c.shift_warm);
     // time-varying problem data on per-instance systems: when the weights keep H positive definite for ANY (Ad, Bd),
     // bmpc_update_problem may defer the condense to the launches that need it
-    h->sys_lazy = false;
+    h->sys_lazy = ns > 1 && weights_keep_h_definite(d, in.data() + P[2].off, ns, o.pw);     // Qx .. QDu (inputs 2..5) are contiguous
     if (ns > 1) {
-        h->sys_lazy = true;
-        for (int si = 0; si < ns && h->sys_lazy; si++) h->sys_lazy = weights_keep_h_definite(d, in.data() + (size_t)si * o.pw + o.Qx);
         if (!h->sys_gen) BMPC_CUDA(cudaMalloc((void**)&h->sys_gen, sizeof(int32_t) * (size_t)ns));
         BMPC_CUDA(cudaMemsetAsync(h->sys_gen, 0, sizeof(int32_t) * (size_t)ns, h->stream));
     }
-    h->sys_gen_cur = 0; h->sys_stale = false; h->sys_bad = false;
+    h->sys_gen_cur = 0; h->sys_stale = false;
+    rc = check_condensed(h, "bmpc_setup");
+    if (rc) return rc;
+    h->sys_bad = false;
     // uminus1 default = uref for every instance (mpc.py:141); caller overrides through bmpc_update
     h->is_setup = true; h->cold = true; h->solved = false; h->pending = false; h->codes_valid = false;
     return BMPC_OK;
@@ -1680,22 +1704,6 @@ int bmpc_update(bmpc_handle* h, const double* x0, const double* uminus1, const d
     return BMPC_OK;
 }
 
-// condensed Hessians of all n_sys systems positive definite (the check of bmpc_setup); otherwise solves are refused until the next
-// successful bmpc_update_system / bmpc_setup
-static int check_condensed(bmpc_handle* h) {
-    const int ns = h->cfg.n_sys; const BmpcSysOff& o = h->o;
-    std::vector<double> errs(ns);
-    BMPC_CUDA(cudaMemcpy2DAsync(errs.data(), sizeof(double), h->sys + o.scal + BMPC_S_ERR, sizeof(double) * o.total, sizeof(double), ns,
-                                cudaMemcpyDeviceToHost, h->stream));
-    BMPC_CUDA(cudaStreamSynchronize(h->stream));
-    for (int si = 0; si < ns; si++) if (errs[si] != 0.0) {
-        h->sys_bad = true;
-        h->err = "bmpc_update_problem: condensed Hessian is not positive definite (the new weights or (Ad, Bd) make the QP non-strictly convex in U)";
-        return BMPC_ERR_NOT_PD;
-    }
-    return BMPC_OK;
-}
-
 int bmpc_update_problem(bmpc_handle* h, const double* Ad, const double* Bd, const double* Qx, const double* QxN, const double* Qu,
                         const double* QDu, const double* xmin, const double* xmax, const double* umin, const double* umax,
                         const double* Dumin, const double* Dumax, const double* uref, int on_device) {
@@ -1705,35 +1713,25 @@ int bmpc_update_problem(bmpc_handle* h, const double* Ad, const double* Bd, cons
     BMPC_CUDA(cudaSetDevice(h->cfg.device));
     if (h->pending) { int rc = finish_solve(h); if (rc) return rc; }
     const BmpcDims& d = h->d; const BmpcSysOff& o = h->o;
-    // the arrays of bmpc_setup in argument order: source, block offset, doubles per system
     const double* src[13] = {Ad, Bd, Qx, QxN, Qu, QDu, xmin, xmax, umin, umax, Dumin, Dumax, uref};
-    const int off[13] = {o.Ad, o.Bd, o.Qx, o.QxN, o.Qu, o.QDu, o.xmin, o.xmax, o.umin, o.umax, o.Dumin, o.Dumax, o.uref};
-    const int cnt[13] = {d.nx * d.nx, d.nx * d.nu, d.nx * d.nx, d.nx * d.nx, d.nu * d.nu, d.nu * d.nu, d.nx, d.nx, d.nu, d.nu, d.nu, d.nu, d.nu};
+    const auto P = problem_inputs(d, o);
     bool any = false;
-    for (int f = 0; f < 13; f++) any = any || src[f];
+    for (const double* s : src) any = any || s;
     if (!any) return BMPC_OK;
     const bool model = Ad || Bd, weights = Qx || QxN || Qu || QDu;
     if (h->cfg.n_sys <= 1) {
         // shared system: eager.  New inputs into the block, K1 with the kept rho, the check of bmpc_setup, then everything that was
-        // derived from the condensed block on the host: the fast paths' constant-bank parameters and the choice of the multi-input entry
-        // (a pattern that leaves the compiled masks, or a QDu that stops being diagonal, must not be answered by k_tpm_pol)
+        // derived from the condensed block on the host
         const cudaMemcpyKind kind = on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
         for (int f = 0; f < 13; f++)
-            if (src[f]) BMPC_CUDA(cudaMemcpyAsync(h->sys + off[f], src[f], sizeof(double) * cnt[f], kind, h->stream));
+            if (src[f]) BMPC_CUDA(cudaMemcpyAsync(h->sys + P[f].off, src[f], sizeof(double) * P[f].cnt, kind, h->stream));
         k_condense_list<<<1, 256, 0, h->stream>>>(d, o, h->sys, 0, nullptr, 1, nullptr, 0, h->cfg.sigma, h->cfg.alpha, h->cfg.eps_feas,
                                                   h->cfg.soft_on, nullptr);
         BMPC_CUDA(cudaGetLastError());
-        int rc = check_condensed(h);
+        int rc = check_condensed(h, "bmpc_update_problem");
         if (rc) return rc;
-        std::vector<double> hs(o.total);
-        BMPC_CUDA(cudaMemcpyAsync(hs.data(), h->sys, sizeof(double) * o.total, cudaMemcpyDeviceToHost, h->stream));
-        BMPC_CUDA(cudaStreamSynchronize(h->stream));
-        if (h->tpi_kind) g_tpi_table[h->tpi_kind - 1].fill(hs.data(), o, h->tpi_admm_params, h->tpi_polish_params);
-        const int old = h->tpm_kind;
-        const int tk = tpm_eligible(h) ? tpm_match(h, hs.data()) : 0;
-        h->tpm_kind = 0;
-        if (tk) { rc = tpm_prepare(h, hs.data(), tk, tk != old); if (rc) return rc; }
-        h->policy.family = policy_family(h);
+        rc = derive_from_block(h, false);
+        if (rc) return rc;
         h->sys_bad = false;
         return BMPC_OK;
     }
@@ -1748,13 +1746,13 @@ int bmpc_update_problem(bmpc_handle* h, const double* Ad, const double* Bd, cons
         if (!src[f]) continue;
         const double* s = src[f];
         if (!on_device) {
-            BMPC_CUDA(cudaMemcpyAsync(h->sys_stage + (size_t)B * off[f], s, sizeof(double) * B * cnt[f], cudaMemcpyHostToDevice, h->stream));
-            s = h->sys_stage + (size_t)B * off[f];
+            BMPC_CUDA(cudaMemcpyAsync(h->sys_stage + (size_t)B * P[f].off, s, sizeof(double) * B * P[f].cnt, cudaMemcpyHostToDevice, h->stream));
+            s = h->sys_stage + (size_t)B * P[f].off;
         }
         const int view = !te ? -1 : f == 0 ? te->view_ad : f == 1 ? te->view_bd : -1;
         view_fill = view_fill || (te && f >= 2);
-        T.seg[T.n++] = BmpcRefreshSeg{s, off[f], cnt[f], view};
-        per += (size_t)cnt[f];
+        T.seg[T.n++] = BmpcRefreshSeg{s, P[f].off, P[f].cnt, view};
+        per += (size_t)P[f].cnt;
     }
     const size_t n = (size_t)B * per;
     k_sys_refresh<<<(unsigned)((n + 255) / 256), 256, 0, h->stream>>>(h->sys, h->I.sys_stride, B, T, h->tpi_view);
@@ -1766,19 +1764,18 @@ int bmpc_update_problem(bmpc_handle* h, const double* Ad, const double* Bd, cons
     bool check = model && !h->sys_lazy;
     if (weights && on_device) { h->sys_lazy = false; check = true; }
     else if (weights) {
-        const int nw = o.xmin - o.Qx;                     // Qx, QxN, Qu, QDu are contiguous in the block
+        const int w0 = P[2].off, nw = P[5].off + P[5].cnt - w0;     // Qx, QxN, Qu, QDu (inputs 2..5) are contiguous in the block
         std::vector<double> w((size_t)B * nw);
-        BMPC_CUDA(cudaMemcpy2DAsync(w.data(), sizeof(double) * nw, h->sys + o.Qx, sizeof(double) * h->I.sys_stride, sizeof(double) * nw, B,
+        BMPC_CUDA(cudaMemcpy2DAsync(w.data(), sizeof(double) * nw, h->sys + w0, sizeof(double) * h->I.sys_stride, sizeof(double) * nw, B,
                                     cudaMemcpyDeviceToHost, h->stream));
         BMPC_CUDA(cudaStreamSynchronize(h->stream));
-        h->sys_lazy = true;
-        for (int si = 0; si < B && h->sys_lazy; si++) h->sys_lazy = weights_keep_h_definite(d, w.data() + (size_t)si * nw);
+        h->sys_lazy = weights_keep_h_definite(d, w.data(), B, nw);
         check = !h->sys_lazy;
     }
     if (check) {
         condense_stale(h, nullptr, B, nullptr);
         BMPC_CUDA(cudaGetLastError());
-        int rc = check_condensed(h);
+        int rc = check_condensed(h, "bmpc_update_problem");
         if (rc) return rc;
     }
     // (bounds and uref alone leave definiteness as it was: a handle refused after a failed update stays refused)
@@ -1963,7 +1960,7 @@ static int finish_solve(bmpc_handle* h) {
 int bmpc_solve(bmpc_handle* h) {
     if (!h) return BMPC_ERR_ARG;
     if (!h->is_setup) { h->err = "bmpc_solve before bmpc_setup"; return BMPC_ERR_STATE; }
-    if (h->sys_bad) { h->err = "bmpc_solve after a failed bmpc_update_system / bmpc_update_problem (condensed Hessian not positive definite): update again or set up anew"; return BMPC_ERR_STATE; }
+    if (h->sys_bad) { h->err = "bmpc_solve after a failed bmpc_setup / bmpc_update_problem / bmpc_update_system (condensed Hessian not positive definite): update again or set up anew"; return BMPC_ERR_STATE; }
     BMPC_CUDA(cudaSetDevice(h->cfg.device));
     if (h->pending) { int rc = finish_solve(h); if (rc) return rc; }
     const int B = h->cfg.batch;

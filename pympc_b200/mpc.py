@@ -125,7 +125,7 @@ class MPCController:
         self._per_instance = batch is not None and Ad.ndim == 3
         if self._per_instance:
             if Ad.shape[0] != int(batch) or Ad.shape[1] != Ad.shape[2]:
-                raise ValueError("Ad should be a square matrix of dimension (nx,nx)!")
+                raise ValueError(self._MSG["Ad"])
             self._sys_full = dict(Ad=Ad, Bd=Bd, Qx=Qx, QxN=QxN, Qu=Qu, QDu=QDu, xmin=xmin, xmax=xmax, umin=umin, umax=umax,
                                   Dumin=Dumin, Dumax=Dumax)
             pick = lambda a, nd: None if a is None else (np.asarray(a)[0] if np.ndim(a) == nd + 1 else a)
@@ -136,12 +136,12 @@ class MPCController:
             self.Ad = Ad
             self.nx = Ad.shape[0]
         else:
-            raise ValueError("Ad should be a square matrix of dimension (nx,nx)!")
+            raise ValueError(self._MSG["Ad"])
         if __is_matrix__(Bd) and Bd.shape[0] == self.nx:
             self.Bd = Bd
             self.nu = Bd.shape[1]
         else:
-            raise ValueError("Bd should be a matrix of dimension (nx, nu)!")
+            raise ValueError(self._MSG["Bd"])
         if Np > 1:
             self.Np = Np
         else:
@@ -168,37 +168,37 @@ class MPCController:
             if __is_vector__(uref) and uref.size == nu:
                 self.uref = uref.ravel()
             else:
-                raise ValueError("uref should be a vector of shape (nu,)!")
+                raise ValueError(self._MSG["uref"])
         else:
             self.uref = np.zeros(nu)
         self.uminus1 = self._vec_or_batch(uminus1, nu, "uminus1 should be a vector of shape (nu,)!", self.uref)
 
-        def weight(Q, n, msg, default):
+        def weight(name, Q, n, default):
             if Q is None:
                 return default
             Qd = Q if hasattr(Q, "toarray") else np.asarray(Q)
             if Qd.ndim == 2 and Qd.shape[0] == n and Qd.shape[1] == n:
                 return Q
-            raise ValueError(msg)
-        self.Qx = weight(Qx, nx, "Qx should be a matrix of shape (nx, nx)!", np.zeros((nx, nx)))   # zeros, not eye (mpc.py:150)
-        self.QxN = weight(QxN, nx, "QxN should be a square matrix of shape (nx, nx)!", self.Qx)
-        self.Qu = weight(Qu, nu, "Qu should be a square matrix of shape (nu, nu)!", np.zeros((nu, nu)))
-        self.QDu = weight(QDu, nu, "QDu should be a square matrix of shape (nu, nu)!", np.zeros((nu, nu)))
+            raise ValueError(self._MSG[name])
+        self.Qx = weight("Qx", Qx, nx, np.zeros((nx, nx)))   # zeros, not eye (mpc.py:150)
+        self.QxN = weight("QxN", QxN, nx, self.Qx)
+        self.Qu = weight("Qu", Qu, nu, np.zeros((nu, nu)))
+        self.QDu = weight("QDu", QDu, nu, np.zeros((nu, nu)))
 
-        def bound(v, n, msg, default):
+        def bound(name, v, n, default):
             if v is None:
                 return default
             v = np.asarray(v, dtype=float)
             if __is_vector__(v) and v.size == n:
                 return v.ravel()
-            raise ValueError(msg)
+            raise ValueError(self._MSG[name])
         inf = np.inf
-        self.xmin = bound(xmin, nx, "xmin should be a vector of shape (nx,)!", -np.ones(nx) * inf)
-        self.xmax = bound(xmax, nx, "xmax should be a vector of shape (nx,)!", np.ones(nx) * inf)
-        self.umin = bound(umin, nu, "umin should be a vector of shape (nu,)!", -np.ones(nu) * inf)
-        self.umax = bound(umax, nu, "umax should be a vector of shape (nu,)!", np.ones(nu) * inf)
-        self.Dumin = bound(Dumin, nu, "Dumin should be a vector of shape (nu,)!", -np.ones(nu) * inf)
-        self.Dumax = bound(Dumax, nu, "Dumax should be a vector of shape (nu,)!", np.ones(nu) * inf)
+        self.xmin = bound("xmin", xmin, nx, -np.ones(nx) * inf)
+        self.xmax = bound("xmax", xmax, nx, np.ones(nx) * inf)
+        self.umin = bound("umin", umin, nu, -np.ones(nu) * inf)
+        self.umax = bound("umax", umax, nu, np.ones(nu) * inf)
+        self.Dumin = bound("Dumin", Dumin, nu, -np.ones(nu) * inf)
+        self.Dumax = bound("Dumax", Dumax, nu, np.ones(nu) * inf)
 
         self.eps_feas = eps_feas
         self.Qeps = eps_feas * np.eye(nx)
@@ -230,6 +230,7 @@ class MPCController:
         self.x0_rh = None
         self.uminus1_rh = None
         self._J_CNST = None
+        self._w_full = {}
         self._J_dirty = True
         self._pin = {}
         self._pin_flip = {}
@@ -350,30 +351,8 @@ class MPCController:
             msg = L.bmpc_last_error(None)
             raise BmpcError(f"bmpc_create failed ({rc}): {msg.decode() if msg else ''}")
         self._h = h
-        z = np.zeros
-        Qx = _dense(self.Qx) if self.JX_ON else z((nx, nx))
-        QxN = _dense(self.QxN) if self.JX_ON else z((nx, nx))
-        Qu = _dense(self.Qu) if self.JU_ON else z((nu, nu))
-        QDu = _dense(self.QDu) if self.JDU_ON else z((nu, nu))
-        args = [np.ascontiguousarray(a, dtype=float) for a in
-                (self.Ad, self.Bd, Qx, QxN, Qu, QDu, self.xmin, self.xmax, self.umin, self.umax, self.Dumin, self.Dumax, self.uref)]
-        if self._per_instance:
-            # every system array gets a leading batch dimension (shared ones are broadcast)
-            full = self._sys_full
-            def per(name, shared, nd, on=True):
-                a = full.get(name)
-                a = shared if (a is None or np.ndim(a) != nd + 1) else np.asarray(a, dtype=float)
-                a = np.broadcast_to(np.asarray(a, dtype=float), (B,) + np.shape(shared))
-                return np.ascontiguousarray(a if on else 0 * a)
-            args = [per("Ad", args[0], 2), per("Bd", args[1], 2), per("Qx", _dense(self.Qx), 2, self.JX_ON),
-                    per("QxN", _dense(self.QxN), 2, self.JX_ON), per("Qu", _dense(self.Qu), 2, self.JU_ON),
-                    per("QDu", _dense(self.QDu), 2, self.JDU_ON), per("xmin", args[6], 1), per("xmax", args[7], 1),
-                    per("umin", args[8], 1), per("umax", args[9], 1), per("Dumin", args[10], 1), per("Dumax", args[11], 1),
-                    per("uref", self.uref, 1)]
-        self._check(L.bmpc_setup(self._h, *[ptr(a) for a in args]))
-        self._Qx_d, self._QxN_d, self._Qu_d, self._QDu_d = Qx, QxN, Qu, QDu
-        # per-instance controllers: every instance's weights as sent to the device (J_CNST)
-        self._w_full = dict(zip(("Qx", "QxN", "Qu", "QDu"), args[2:6])) if self._per_instance else {}
+        sent = self._device_arrays(self._setup_arrays())
+        self._check(L.bmpc_setup(self._h, *[ptr(sent[name]) for name, _, _ in self._PROBLEM]))
         self._qp_static = None
         self._um1_for_J = self.uminus1_rh
         self._push(self.x0_rh, self.uminus1_rh, self.xref)
@@ -484,6 +463,37 @@ class MPCController:
         return {"Ad": (nx, nx), "Bd": (nx, nu), "Qx": (nx, nx), "QxN": (nx, nx), "Qu": (nu, nu), "QDu": (nu, nu)}.get(
             name, (nx,) if name in ("xmin", "xmax") else (nu,))
 
+    def _setup_arrays(self):
+        """the 13 arrays setup() hands the library, by name: the attributes; per-instance controllers take an array given with a
+        leading batch dimension (at construction or by update_system) over the attribute, which then holds instance 0's"""
+        arrays = {name: getattr(self, name) for name, _, _ in self._PROBLEM}
+        if self._per_instance:
+            for name, _, _ in self._PROBLEM:
+                full = self._sys_full.get(name)
+                if full is not None and np.ndim(full) == len(self._problem_shape(name)) + 1:
+                    arrays[name] = full
+        return arrays
+
+    def _device_arrays(self, arrays):
+        """{name: array} of bmpc_setup / bmpc_update_problem -> the arrays the library receives: float64 and C-contiguous, a weight
+        whose JX_ON / JU_ON / JDU_ON is off as zeros, and on per-instance controllers with a leading batch dimension (an array given
+        once is broadcast to every instance).  Records the weights sent: _Qx_d ... _QDu_d (instance 0's; the reference-form QP)
+        and on per-instance controllers every instance's in _w_full (J_CNST)."""
+        B, per = self._B, self._per_instance
+        sent = {}
+        for name, kind, flag in self._PROBLEM:
+            if name not in arrays:
+                continue
+            M = _dense(arrays[name])
+            if flag is not None and not getattr(self, flag):
+                M = np.zeros(M.shape)
+            sent[name] = np.ascontiguousarray(np.broadcast_to(M, (B,) + self._problem_shape(name))) if per else M
+            if kind == "weight":
+                setattr(self, "_" + name + "_d", sent[name][0] if per else sent[name])
+                if per:
+                    self._w_full[name] = sent[name]
+        return sent
+
     def update_system(self, Ad=None, Bd=None, *, Qx=None, QxN=None, Qu=None, QDu=None, xmin=None, xmax=None, umin=None, umax=None,
                       Dumin=None, Dumax=None, uref=None):
         """Time-varying problem data (successive linearisation, gain scheduling, derated actuator limits, tightened constraints):
@@ -496,7 +506,7 @@ class MPCController:
         set per instance.  Matrices dense or scipy.sparse.  None keeps an array.  JX_ON / JU_ON / JDU_ON zero the weights sent to
         the device as in setup().  The reference-form attributes (Ad, ..., uref, P, q, A, l, u, J_CNST) and u_failure follow;
         assigning ``K.xmin = ...`` directly keeps the reference's meaning: no effect until setup()."""
-        B, per = self._B, self._per_instance
+        per = self._per_instance
         vals = dict(Ad=Ad, Bd=Bd, Qx=Qx, QxN=QxN, Qu=Qu, QDu=QDu, xmin=xmin, xmax=xmax, umin=umin, umax=umax, Dumin=Dumin, Dumax=Dumax,
                     uref=uref)
         given = {name: self._problem_arg(vals[name], name) for name, _, _ in self._PROBLEM if vals[name] is not None}
@@ -504,14 +514,7 @@ class MPCController:
             raise BmpcError("update_system() before setup()")
         if not given:
             return
-        sent = {}
-        for name, kind, flag in self._PROBLEM:
-            if name not in given:
-                continue
-            M = given[name]
-            if flag is not None and not getattr(self, flag):
-                M = np.zeros(M.shape)
-            sent[name] = np.ascontiguousarray(np.broadcast_to(M, (B,) + self._problem_shape(name))) if per else M
+        sent = self._device_arrays(given)
         args = [ptr(sent[name]) if name in sent else None for name, _, _ in self._PROBLEM]
         if set(given) <= {"Ad", "Bd"}:
             rc = self._L.bmpc_update_system(self._h, args[0], args[1], 0)
@@ -527,9 +530,6 @@ class MPCController:
                 self._sys_full[name] = M
             if kind == "weight":
                 setattr(self, name, M[0] if full else (vals[name] if hasattr(vals[name], "toarray") else M))   # (sparse stays sparse, Q16)
-                setattr(self, "_" + name + "_d", sent[name][0] if per else sent[name])
-                if per:
-                    self._w_full[name] = sent[name]
             else:
                 setattr(self, name, M[0] if full else M)
             if name == "uref":
