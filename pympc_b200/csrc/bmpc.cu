@@ -1065,9 +1065,8 @@ struct bmpc_handle {
     bmpc_config cfg;
     BmpcDims d;
     BmpcSysOff o;
-    int team;        // 32 or CTA size
-    int wpb;         // warps per block (warp team)
-    int rmax;
+    BmpcLaunch launch = {};            // team size, polish tiers and tile size (bmpc_plan_launch); each team round: bmpc_round_launch
+    int sm_count = 132;
     cudaStream_t stream, own_stream;
     double* sys = nullptr;
     BmpcInst I;
@@ -1089,15 +1088,9 @@ struct bmpc_handle {
     bool is_setup = false, cold = true, solved = false, committed = true;   // committed: this solve's u0 already is the next u_-1
     bmpc_stats stats;
     std::string err;
-    size_t smem_admm = 0, smem_polish = 0;
-    // low-latency CTA-per-instance variant for the few stragglers of a warp-team / TPI handle
-    int fb_team = 0, fb_rmax = 0; size_t fb_smem_polish = 0;
-    bool fb_overflow = false;          // the warp-team polish hands working sets beyond rmax to this CTA tier in the same round
-    int rmax_small = 0; size_t smem_polish_small = 0; int32_t* ovf = nullptr;   // small-capacity polish tier (CTA teams) + its overflow list
-    int sm_count = 132;
+    int32_t* ovf = nullptr;            // overflow list of the first polish tier, read by the second
     double* vprev = nullptr; int32_t* lprev = nullptr;   // snapshot of (v, level) for the infeasibility check of straggler rounds
-    void (*tile_fn[3])(BmpcDims, BmpcSysOff, const double*, BmpcInst, const int32_t*, int, int, int, int, int, int) = {nullptr, nullptr, nullptr};
-    int tile_T = 0, tile_threads = 0;                  // > 0: the ADMM of this shape runs on tiles of T instances per CTA
+    void (*tile_fn[3])(BmpcDims, BmpcSysOff, const double*, BmpcInst, const int32_t*, int, int, int, int, int, int) = {nullptr, nullptr, nullptr};   // tiles of 8, 4, 2
     struct { const int32_t* list; int count; int32_t *cur, *nxt; int total, chunk, round; bool need_prep; int tight; bool cold; } st = {};
     bool pending = false;              // a round is in flight and has not been retired by the host yet
     int tpi_kind = 0;                  // 0 none, else 1 + index into g_tpi_table (compiled fast-path shapes)
@@ -1306,29 +1299,24 @@ static int configure_launch(bmpc_handle* h) {
     cudaDeviceGetAttribute(&max_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
     cudaDeviceGetAttribute(&h->sm_count, cudaDevAttrMultiProcessorCount, dev);
     // team size, tiers and tile size: one decision the host emulation shares (bmpc_launch.cuh)
-    const BmpcLaunch L = bmpc_plan_launch(d, max_optin, h->cfg.team_threads, h->cfg.warps_per_block, h->cfg.rmax, h->cfg.n_sys);
+    const BmpcLaunch& L = h->launch = bmpc_plan_launch(d, max_optin, h->cfg.team_threads, h->cfg.warps_per_block, h->cfg.rmax, h->cfg.n_sys);
     if (!L.ok) { h->err = "problem too large for the shared-memory resident kernels"; return BMPC_ERR_ARG; }
-    h->team = L.team; h->wpb = L.wpb; h->rmax = L.rmax;
-    h->smem_admm = L.smem_admm; h->smem_polish = L.smem_polish;
-    h->fb_team = L.fb_team; h->fb_rmax = L.fb_rmax; h->fb_smem_polish = L.fb_smem_polish; h->fb_overflow = L.overflow != 0;
-    h->rmax_small = L.rmax_small; h->smem_polish_small = L.smem_polish_small;
-    h->tile_T = L.tile_T; h->tile_threads = L.tile_threads;
-    if (h->tile_T) {
+    if (L.tile_T) {
         // kernels per tile size {8, 4, 2}; shapes with a compiled (nx, nu) get the unrolled instantiation
         if (d.nx == 8 && d.nu == 4) { h->tile_fn[0] = k_admm_tile<8, 2, 8, 4>; h->tile_fn[1] = k_admm_tile<4, 2, 8, 4>; h->tile_fn[2] = k_admm_tile<2, 1, 8, 4>; }
         else { h->tile_fn[0] = k_admm_tile<8, 2, 0, 0>; h->tile_fn[1] = k_admm_tile<4, 2, 0, 0>; h->tile_fn[2] = k_admm_tile<2, 1, 0, 0>; }
         for (int k = 0; k < 3; k++) {
             const int T = 8 >> k;
-            if (h->tile_T >= T) BMPC_CUDA(cudaFuncSetAttribute((const void*)h->tile_fn[k], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(bmpc_tile_smem_doubles(d, T) * 8)));
+            if (L.tile_T >= T) BMPC_CUDA(cudaFuncSetAttribute((const void*)h->tile_fn[k], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(bmpc_tile_smem_doubles(d, T) * 8)));
         }
     }
-    if (h->team == 32) {
-        BMPC_CUDA(cudaFuncSetAttribute(k_admm<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_admm));
-        BMPC_CUDA(cudaFuncSetAttribute(k_polish<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_polish));
-        if (h->fb_team) BMPC_CUDA(cudaFuncSetAttribute(k_polish<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->fb_smem_polish));
+    if (L.team == 32) {
+        BMPC_CUDA(cudaFuncSetAttribute(k_admm<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.smem_admm));
+        BMPC_CUDA(cudaFuncSetAttribute(k_polish<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.smem_polish));
+        if (L.fb_team) BMPC_CUDA(cudaFuncSetAttribute(k_polish<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.fb_smem_polish));
     } else {
-        BMPC_CUDA(cudaFuncSetAttribute(k_admm<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_admm));
-        BMPC_CUDA(cudaFuncSetAttribute(k_polish<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_polish));
+        BMPC_CUDA(cudaFuncSetAttribute(k_admm<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.smem_admm));
+        BMPC_CUDA(cudaFuncSetAttribute(k_polish<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.smem_polish));
     }
     return BMPC_OK;
 }
@@ -1487,7 +1475,7 @@ int bmpc_gather_arrive(bmpc_handle* h, int64_t epoch) {
 int bmpc_get_dims(const bmpc_handle* h, int32_t* dims) {
     if (!h || !dims) return BMPC_ERR_ARG;
     dims[0] = h->d.nx; dims[1] = h->d.nu; dims[2] = h->d.Np; dims[3] = h->d.Nc; dims[4] = h->d.NX; dims[5] = h->d.NU;
-    dims[6] = h->d.mc; dims[7] = h->team;
+    dims[6] = h->d.mc; dims[7] = h->launch.team;
     return BMPC_OK;
 }
 
@@ -1640,7 +1628,7 @@ int bmpc_setup(bmpc_handle* h, const double* Ad, const double* Bd, const double*
     // blocks hold, so a later update decides and refreshes from the same state as after a failed update
     // thread-per-instance fast path for the compiled small shapes (pendulum, point mass)
     // (the Riccati polish treats state rows as the soft penalty they are by default; hard state rows -> team kernels)
-    h->tpi_kind = h->cfg.fast_path && h->team == 32 && h->cfg.soft_on ? find_shape(g_tpi_table, g_tpi_count, d) + 1 : 0;
+    h->tpi_kind = h->cfg.fast_path && h->launch.team == 32 && h->cfg.soft_on ? find_shape(g_tpi_table, g_tpi_count, d) + 1 : 0;
     if (h->tpi_kind) {
         const TpiEntry& te = g_tpi_table[h->tpi_kind - 1];
         if (te.code_stride > h->code_stride) { h->err = "fast path: working-set record larger than allocated"; return BMPC_ERR_STATE; }
@@ -1787,54 +1775,32 @@ int bmpc_update_system(bmpc_handle* h, const double* Ad, const double* Bd, int o
     return bmpc_update_problem(h, Ad, Bd, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, on_device);
 }
 
-static bool use_fallback_team(const bmpc_handle* h, const int32_t* list, int count) {
-    return h->team == 32 && h->fb_team && list != nullptr && count <= BMPC_FB_MAX_LIST;
-}
-
-static void launch_admm(bmpc_handle* h, const int32_t* list, int count, int niter, int do_prep) {
-    const int cold = h->cold ? 1 : 0;
-    if (use_fallback_team(h, list, count)) {
-        // stragglers of a warp-team / fast-path handle: one warp per CTA (the lanes-own-rows ADMM has the shortest
-        // dependent chain per iteration for these small shapes: measured 5 % on the random-instance bench vs a 128-thread CTA)
-        k_admm<true><<<count, 32, bmpc_admm_smem_doubles(h->d) * 8, h->stream>>>(h->d, h->o, h->sys, h->I, list, count, niter, do_prep, cold, h->xref_mode, h->cfg.polish ? 1 : 0);
-    } else if (h->team == 32 && h->tile_T == 0) {
-        int grid = (count + h->wpb - 1) / h->wpb;
-        k_admm<true><<<grid, h->wpb * 32, h->smem_admm, h->stream>>>(h->d, h->o, h->sys, h->I, list, count, niter, do_prep, cold, h->xref_mode, h->cfg.polish ? 1 : 0);
-    } else if (h->tile_T > 0) {
-        // throughput tiles (8 instances share every K^-1 entry) while the batch fills the GPU twice over; straggler rounds
-        // with few instances left use small tiles: more CTAs, a shorter dependent chain per iteration
-        int k = (h->tile_T == 8 && count > 2 * h->sm_count * 8) ? 0 : ((h->tile_T >= 4 && count > 2 * h->sm_count * 2) ? 1 : 2);
-        while ((8 >> k) > h->tile_T) k++;
-        const int T = 8 >> k;
-        h->tile_fn[k]<<<(count + T - 1) / T, h->tile_threads, bmpc_tile_smem_doubles(h->d, T) * 8, h->stream>>>(h->d, h->o, h->sys, h->I, list, count, niter, do_prep, cold, h->xref_mode, h->cfg.polish ? 1 : 0);
-    } else {
-        k_admm<false><<<count, h->team, h->smem_admm, h->stream>>>(h->d, h->o, h->sys, h->I, list, count, niter, do_prep, cold, h->xref_mode, h->cfg.polish ? 1 : 0);
+static void launch_admm(bmpc_handle* h, const BmpcRoundLaunch& R, const int32_t* list, int count, int niter, int do_prep) {
+    const int cold = h->cold ? 1 : 0, polish = h->cfg.polish ? 1 : 0;
+    switch (R.admm) {
+    case BMPC_TADMM_WARP: case BMPC_TADMM_LONE_WARP:
+        k_admm<true><<<R.admm_grid, R.admm_threads, R.admm_smem, h->stream>>>(h->d, h->o, h->sys, h->I, list, count, niter, do_prep, cold, h->xref_mode, polish);
+        break;
+    case BMPC_TADMM_TILE:
+        h->tile_fn[R.tile_T == 8 ? 0 : R.tile_T == 4 ? 1 : 2]<<<R.admm_grid, R.admm_threads, R.admm_smem, h->stream>>>(h->d, h->o, h->sys, h->I, list, count, niter, do_prep, cold, h->xref_mode, polish);
+        break;
+    case BMPC_TADMM_CTA:
+        k_admm<false><<<R.admm_grid, R.admm_threads, R.admm_smem, h->stream>>>(h->d, h->o, h->sys, h->I, list, count, niter, do_prep, cold, h->xref_mode, polish);
+        break;
     }
     h->stats.launches++;
 }
 
-static void launch_polish(bmpc_handle* h, const int32_t* list, int count, int steps, int32_t* next_list, int32_t* next_count) {
-    if (use_fallback_team(h, list, count)) {
-        k_polish<false><<<count, h->fb_team, h->fb_smem_polish, h->stream>>>(h->d, h->o, h->sys, h->I, list, count, h->fb_rmax, steps, next_list, next_count, h->I.u0, nullptr, nullptr, h->cfg.candidate_warm);
-    } else if (h->team == 32) {
-        // working sets beyond the warp tier go to the CTA tier right after (count read on the device): whether an instance can be
-        // verified must not depend on how many instances are open
-        int grid = (count + h->wpb - 1) / h->wpb;
-        k_polish<true><<<grid, h->wpb * 32, h->smem_polish, h->stream>>>(h->d, h->o, h->sys, h->I, list, count, h->rmax, steps, next_list, next_count, h->I.u0, nullptr, h->fb_overflow ? h->ovf : nullptr, h->cfg.candidate_warm);
-        if (h->fb_overflow) {
-            k_polish<false><<<count, h->fb_team, h->fb_smem_polish, h->stream>>>(h->d, h->o, h->sys, h->I, h->ovf, count, h->fb_rmax, steps, next_list, next_count, h->I.u0, next_count + 2, nullptr, h->cfg.candidate_warm);
-            h->stats.launches++;
-        }
-    } else if (h->rmax_small > 0) {
-        // two capacity tiers: the small one keeps several CTAs resident per SM (the polish is latency-bound); working
-        // sets that outgrow it are listed and redone by the full-capacity launch right after (count read on the device)
-        k_polish<false><<<count, h->team, h->smem_polish_small, h->stream>>>(h->d, h->o, h->sys, h->I, list, count, h->rmax_small, steps, next_list, next_count, h->I.u0, nullptr, h->ovf, h->cfg.candidate_warm);
-        k_polish<false><<<count, h->team, h->smem_polish, h->stream>>>(h->d, h->o, h->sys, h->I, h->ovf, count, h->rmax, steps, next_list, next_count, h->I.u0, next_count + 2, nullptr, h->cfg.candidate_warm);
+static void launch_polish(bmpc_handle* h, const BmpcRoundLaunch& R, const int32_t* list, int count, int steps, int32_t* next_list, int32_t* next_count) {
+    for (int k = 0; k < R.ntiers; k++) {
+        const BmpcPolishTier& t = R.tier[k];
+        const int32_t* tlist = k == 0 ? list : h->ovf;
+        const int32_t* dev_count = k == 0 ? nullptr : next_count + 2;     // filled by the tier before
+        int32_t* ovf = k + 1 < R.ntiers ? h->ovf : nullptr;
+        if (t.warp) k_polish<true><<<t.grid, t.threads, t.smem, h->stream>>>(h->d, h->o, h->sys, h->I, tlist, count, t.rmax, steps, next_list, next_count, h->I.u0, dev_count, ovf, h->cfg.candidate_warm);
+        else k_polish<false><<<t.grid, t.threads, t.smem, h->stream>>>(h->d, h->o, h->sys, h->I, tlist, count, t.rmax, steps, next_list, next_count, h->I.u0, dev_count, ovf, h->cfg.candidate_warm);
         h->stats.launches++;
-    } else {
-        k_polish<false><<<count, h->team, h->smem_polish, h->stream>>>(h->d, h->o, h->sys, h->I, list, count, h->rmax, steps, next_list, next_count, h->I.u0, nullptr, nullptr, h->cfg.candidate_warm);
     }
-    h->stats.launches++;
 }
 
 // ---- solve = rounds of [ADMM chunk -> polish]; the host only needs the count of unfinished instances after each
@@ -1881,8 +1847,9 @@ static int enqueue_round(bmpc_handle* h, const BmpcRoundPlan& p) {
         BMPC_CUDA(cudaEventRecord(h->ev[1], h->stream));
         g_tpm_table[h->tpm_kind - 1].launch(h, st.list, st.count, p.ws, p.cap, p.reset, st.nxt, p.exchange);
     } else {
+        const BmpcRoundLaunch R = bmpc_round_launch(h->launch, h->d, st.count, st.list != nullptr, h->sm_count);
         if (p.infeas) { k_snapshot<<<st.count, 128, 0, h->stream>>>(h->d, h->I, st.list, st.count, h->vprev, h->lprev); h->stats.launches++; }
-        launch_admm(h, st.list, st.count, p.chunk, st.need_prep ? 1 : 0);
+        launch_admm(h, R, st.list, st.count, p.chunk, st.need_prep ? 1 : 0);
         st.need_prep = false;
         if (p.infeas) {
             k_infeas<<<st.count, 128, sizeof(double) * (h->d.mc + h->d.nu + 2), h->stream>>>(h->d, h->o, h->sys, h->I, st.list, st.count, h->vprev, h->lprev, 1e-4, h->I.u0, cnt);
@@ -1891,7 +1858,7 @@ static int enqueue_round(bmpc_handle* h, const BmpcRoundPlan& p) {
         BMPC_CUDA(cudaEventRecord(h->ev[1], h->stream));
         if (p.polish == BMPC_POL_TPI) g_tpi_table[h->tpi_kind - 1].launch(h, st.list, st.count, p, st.nxt);
         else if (p.polish == BMPC_POL_TPM) g_tpm_table[h->tpm_kind - 1].launch(h, st.list, st.count, p.ws, p.cap, 0, st.nxt, p.exchange);
-        else if (p.polish == BMPC_POL_SCHUR) launch_polish(h, st.list, st.count, p.cap, st.nxt, cnt);
+        else if (p.polish == BMPC_POL_SCHUR) launch_polish(h, R, st.list, st.count, p.cap, st.nxt, cnt);
         else { k_check_converged<<<(st.count + 255) / 256, 256, 0, h->stream>>>(h->I, st.list, st.count, h->cfg.eps_abs, h->cfg.eps_rel, st.nxt, cnt); h->stats.launches++; }
     }
     h->I.um1 = h->um1_cur;

@@ -1,7 +1,7 @@
 // bmpc_launch.cuh — launch configuration of the team / tile kernels: team size, instances per CTA, the working-set capacity of
 // every Schur-form polish tier and the tile size of the ADMM.  Host code only, plain C++: libbmpc.so configures a handle with
-// bmpc_plan_launch at bmpc_create and the host emulation (tests/hostemu) runs the same function, so the capacities an instance
-// meets in the emulation are the device's.
+// bmpc_plan_launch at bmpc_create and launches every team round as bmpc_round_launch describes it; the host emulation
+// (tests/hostemu) runs the same functions, so the capacities an instance meets in the emulation are the device's.
 //
 // The polish holds its working set (violated soft rows + active hard rows) in shared memory: its Schur matrix is packed,
 // r(r+1)/2 doubles.  A working set larger than a tier's capacity makes bmpc_polish return -1 and the instance moves to the next
@@ -35,7 +35,8 @@ struct BmpcLaunch {
     size_t smem_admm, smem_polish, smem_polish_small, fb_smem_polish;   // dynamic shared memory per CTA (bytes)
 };
 
-// straggler rounds of a warp-team handle with at most this many instances run on the CTA tier alone (ADMM and polish)
+// straggler rounds of a warp-team handle with at most this many instances run on one warp per CTA (ADMM) and the CTA tier
+// alone (polish): they are latency-bound
 enum { BMPC_FB_MAX_LIST = 4096 };
 
 // largest capacity <= want whose polish fits `budget` bytes (one instance); shrinks to 8 at the least
@@ -88,16 +89,90 @@ inline BmpcLaunch bmpc_plan_launch(const BmpcDims& d, int max_optin, int team_th
     return L;
 }
 
-// capacities of the polish tiers an instance passes through in a round over `count` open instances (list_given: a straggler
-// round; the first round covers the whole batch), smallest first; returns how many (<= 2)
-inline int bmpc_polish_tiers(const BmpcLaunch& L, int count, bool list_given, int* caps) {
-    if (L.team == 32) {
-        if (L.fb_team && list_given && count <= BMPC_FB_MAX_LIST) { caps[0] = L.fb_rmax; return 1; }
-        caps[0] = L.rmax;
-        if (L.overflow) { caps[1] = L.fb_rmax; return 2; }
-        return 1;
+// ADMM kernel of a team round
+enum BmpcTeamAdmm {
+    BMPC_TADMM_WARP,       // k_admm<true>, wpb instances per CTA
+    BMPC_TADMM_LONE_WARP,  // k_admm<true>, one warp per CTA (short straggler lists)
+    BMPC_TADMM_TILE,       // k_admm_tile of tile_T instances per CTA
+    BMPC_TADMM_CTA         // k_admm<false>, one CTA per instance
+};
+
+// one Schur-form polish launch: k_polish<warp>
+struct BmpcPolishTier {
+    int warp;                    // 1: k_polish<true> (a warp per instance), 0: k_polish<false> (a CTA per instance)
+    int grid, threads, rmax;
+    size_t smem;
+};
+
+// the team / tile launches of one round (bmpc_round_launch)
+struct BmpcRoundLaunch {
+    int admm;                    // BmpcTeamAdmm
+    int tile_T;                  // BMPC_TADMM_TILE: instances per CTA (8, 4 or 2)
+    int admm_grid, admm_threads;
+    size_t admm_smem;
+    int ntiers;                  // bmpc_round_polish
+    BmpcPolishTier tier[2];
+};
+
+// a straggler round of a warp-team / fast-path handle short enough for one warp per CTA (ADMM) and the CTA tier alone (polish)
+inline bool bmpc_lone_stragglers(const BmpcLaunch& L, int count, bool list_given) {
+    return L.team == 32 && L.fb_team && list_given && count <= BMPC_FB_MAX_LIST;
+}
+
+// the polish tiers of a round over `count` open instances (list_given: a straggler round; the first round covers the whole batch)
+// of a handle planned as L (L.ok), smallest capacity first; returns how many (1 or 2).  The first tier reads the round's list and
+// count and fills the overflow list only when a second tier follows; the second reads the overflow list and takes its count from
+// the device.
+inline int bmpc_round_polish(const BmpcLaunch& L, int count, bool list_given, BmpcPolishTier* tier) {
+    int n = 0;
+    auto add = [&](int warp, int grid, int threads, int rmax, size_t smem) { tier[n++] = BmpcPolishTier{warp, grid, threads, rmax, smem}; };
+    if (bmpc_lone_stragglers(L, count, list_given)) {
+        add(0, count, L.fb_team, L.fb_rmax, L.fb_smem_polish);
+    } else if (L.team == 32) {
+        // working sets beyond the warp tier go to the CTA tier right after: whether an instance can be verified must not depend
+        // on how many instances are open
+        add(1, (count + L.wpb - 1) / L.wpb, L.wpb * 32, L.rmax, L.smem_polish);
+        if (L.overflow) add(0, count, L.fb_team, L.fb_rmax, L.fb_smem_polish);
+    } else {
+        // two capacity tiers: the small one keeps several CTAs resident per SM (the polish is latency-bound); working sets that
+        // outgrow it are redone by the full tier right after
+        if (L.rmax_small) add(0, count, L.team, L.rmax_small, L.smem_polish_small);
+        add(0, count, L.team, L.rmax, L.smem_polish);
     }
-    if (L.rmax_small) { caps[0] = L.rmax_small; caps[1] = L.rmax; return 2; }
-    caps[0] = L.rmax;
-    return 1;
+    return n;
+}
+
+// capacities of the polish tiers of such a round (bmpc_round_polish), smallest first; returns how many (<= 2)
+inline int bmpc_polish_tiers(const BmpcLaunch& L, int count, bool list_given, int* caps) {
+    BmpcPolishTier tier[2];
+    const int n = bmpc_round_polish(L, count, list_given, tier);
+    for (int k = 0; k < n; k++) caps[k] = tier[k].rmax;
+    return n;
+}
+
+// the launches of a team round over `count` open instances (as bmpc_round_polish) on a GPU of sm_count SMs
+inline BmpcRoundLaunch bmpc_round_launch(const BmpcLaunch& L, const BmpcDims& d, int count, bool list_given, int sm_count) {
+    BmpcRoundLaunch R = {};
+    if (bmpc_lone_stragglers(L, count, list_given)) {
+        // the lanes-own-rows ADMM has the shortest dependent chain per iteration for these small shapes: measured 5 % on the
+        // random-instance bench vs a 128-thread CTA
+        R.admm = BMPC_TADMM_LONE_WARP;
+        R.admm_grid = count; R.admm_threads = 32; R.admm_smem = bmpc_admm_smem_doubles(d) * 8;
+    } else if (L.team == 32) {
+        R.admm = BMPC_TADMM_WARP;
+        R.admm_grid = (count + L.wpb - 1) / L.wpb; R.admm_threads = L.wpb * 32; R.admm_smem = L.smem_admm;
+    } else if (L.tile_T > 0) {
+        // throughput tiles (8 instances share every K^-1 entry) while the batch fills the GPU twice over; straggler rounds with
+        // few instances left use small tiles: more CTAs, a shorter dependent chain per iteration
+        int T = L.tile_T;
+        if (T == 8 && count <= 2 * sm_count * 8) T = 4;
+        if (T == 4 && count <= 2 * sm_count * 2) T = 2;
+        R.admm = BMPC_TADMM_TILE; R.tile_T = T;
+        R.admm_grid = (count + T - 1) / T; R.admm_threads = L.tile_threads; R.admm_smem = bmpc_tile_smem_doubles(d, T) * 8;
+    } else {
+        R.admm = BMPC_TADMM_CTA;
+        R.admm_grid = count; R.admm_threads = L.team; R.admm_smem = L.smem_admm;
+    }
+    R.ntiers = bmpc_round_polish(L, count, list_given, R.tier);
+    return R;
 }

@@ -167,6 +167,8 @@ class EmuSystem:
 
 # opt-in shared memory per block of an H100 (cudaDevAttrMaxSharedMemoryPerBlockOptin), bytes
 H100_OPTIN = 232448
+H100_SMS = 132                  # streaming multiprocessors of an H100 SXM (cudaDevAttrMultiProcessorCount)
+_ADMM_KINDS = ("warp", "lone_warp", "tile", "cta")     # BmpcTeamAdmm
 _LAUNCH_FIELDS = ("ok", "team", "wpb", "rmax", "rmax_small", "fb_team", "fb_rmax", "overflow", "tile_T", "tile_threads",
                   "smem_admm", "smem_polish", "smem_polish_small", "fb_smem_polish")
 
@@ -179,6 +181,21 @@ def plan_launch(nx, nu, Np, Nc=None, max_optin=H100_OPTIN, team_threads=0, warps
     f.argtypes = [ctypes.c_int] * 9 + [ctypes.c_void_p]
     f(nx, nu, Np, Nc or Np, max_optin, team_threads, warps_per_block, rmax, n_sys, _p(out))
     return dict(zip(_LAUNCH_FIELDS, (int(v) for v in out)))
+
+
+def round_launch(nx, nu, Np, Nc=None, count=1, list_given=False, sm_count=H100_SMS, max_optin=H100_OPTIN, team_threads=0,
+                 warps_per_block=0, rmax=0, n_sys=1):
+    """the team / tile launches of one round over `count` open instances (bmpc_launch.cuh: bmpc_round_launch; list_given: a
+    straggler round) as a dict: admm kind, tile size, grid, threads and shared memory of the ADMM, and the polish tiers, smallest
+    capacity first; None for a shape bmpc_create refuses"""
+    L = build(); out = np.zeros(16, np.int64)
+    f = L.emu_round_launch
+    f.argtypes = [ctypes.c_int] * 12 + [ctypes.c_void_p]
+    if not f(nx, nu, Np, Nc or Np, max_optin, team_threads, warps_per_block, rmax, n_sys, count, int(list_given), sm_count, _p(out)):
+        return None
+    v = [int(x) for x in out]
+    tiers = [dict(zip(("warp", "grid", "threads", "rmax", "smem"), v[6 + 5 * k:11 + 5 * k])) for k in range(v[5])]
+    return dict(admm=_ADMM_KINDS[v[0]], tile_T=v[1], admm_grid=v[2], admm_threads=v[3], admm_smem=v[4], tiers=tiers)
 
 
 def launch_tiers(nx, nu, Np, Nc=None, count=1, max_optin=H100_OPTIN, team_threads=0, warps_per_block=0, rmax=0, n_sys=1):

@@ -49,6 +49,24 @@ int emu_polish_tiers(int nx, int nu, int Np, int Nc, int max_optin, int team_thr
     return L.ok ? bmpc_polish_tiers(L, count, list_given != 0, caps) : 0;
 }
 
+// the team / tile launches of one round over `count` open instances (bmpc_round_launch): out[16] = admm, tile_T, admm_grid,
+// admm_threads, admm_smem, ntiers, then per tier warp, grid, threads, rmax, smem; returns 0 (out untouched) for a refused shape
+int emu_round_launch(int nx, int nu, int Np, int Nc, int max_optin, int team_threads, int warps_per_block, int rmax, int n_sys,
+                     int count, int list_given, int sm_count, long long* out) {
+    const BmpcDims d = bmpc_make_dims(nx, nu, Np, Nc);
+    const BmpcLaunch L = bmpc_plan_launch(d, max_optin, team_threads, warps_per_block, rmax, n_sys);
+    if (!L.ok) return 0;
+    const BmpcRoundLaunch R = bmpc_round_launch(L, d, count, list_given != 0, sm_count);
+    const long long v[6] = {R.admm, R.tile_T, R.admm_grid, R.admm_threads, (long long)R.admm_smem, R.ntiers};
+    for (int k = 0; k < 6; k++) out[k] = v[k];
+    for (int k = 0; k < 2; k++) {
+        const BmpcPolishTier& t = R.tier[k];
+        const long long w[5] = {t.warp, t.grid, t.threads, t.rmax, (long long)t.smem};
+        for (int j = 0; j < 5; j++) out[6 + 5 * k + j] = w[j];
+    }
+    return 1;
+}
+
 // one full solve of one instance: rounds of ADMM + polish, like the host loop of the library.  The polish of each round runs
 // its tiers like the device: tiers0 [n0] in the first round, tiers1 [n1] in the straggler rounds, smallest capacity first; a
 // working set beyond one tier's capacity is redone by the next.

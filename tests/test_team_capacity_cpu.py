@@ -1,12 +1,12 @@
-"""CPU: the launch configuration of the team / tile kernels (pympc_b200/csrc/bmpc_launch.cuh: bmpc_plan_launch, bmpc_polish_tiers),
-which libbmpc.so and the host emulation share, pinned at an H100's opt-in shared memory (232 448 bytes per block) for the shapes of
-tests/golden/team_shapes.npz and the shared-memory edges; and host twins of the GPU capacity tests: the device core compiled for
-the CPU (tests/hostemu) replays the device's polish tiers on golden instances whose optimal working sets are known."""
+"""CPU: the launch configuration of the team / tile kernels (pympc_b200/csrc/bmpc_launch.cuh: bmpc_plan_launch, bmpc_round_launch),
+which libbmpc.so and the host emulation share, pinned at an H100's opt-in shared memory (232 448 bytes per block) and 132 SMs for
+the shapes of tests/golden/team_shapes.npz and the shared-memory edges; and host twins of the GPU capacity tests: the device core
+compiled for the CPU (tests/hostemu) replays the device's polish tiers on golden instances whose optimal working sets are known."""
 import numpy as np
 import pytest
 
 from conftest import golden
-from emu import EmuSystem, plan_launch, launch_tiers
+from emu import EmuSystem, plan_launch, launch_tiers, round_launch
 
 SYS_KEYS = ("Ad", "Bd", "Qx", "QxN", "Qu", "QDu", "xmin", "xmax", "umin", "umax", "Dumin", "Dumax", "uref")
 
@@ -60,6 +60,66 @@ def test_first_shape_beyond_shared_memory_is_refused():
     assert plan_launch(8, 4, 313)["ok"] == 1
     assert plan_launch(8, 4, 314)["ok"] == 0
     assert plan_launch(12, 6, 208)["ok"] == 1 and plan_launch(12, 6, 209)["ok"] == 0
+
+
+def _cta(count, *caps, threads=256):
+    return [(0, count, threads, c) for c in caps]
+
+
+# (shape, options, open instances, straggler round) -> ADMM (kind, tile size, grid, threads), polish tiers (warp, grid, threads,
+# capacity), smallest capacity first
+ROUNDS = [
+    # warp team: a straggler list of at most 4 096 runs one warp per CTA and the CTA tier alone; anything else the warp tier with
+    # its overflow to the CTA tier
+    ((7, 1, 20, 20), {}, 65536, False, ("warp", 0, 8192, 256), [(1, 8192, 256, 64)] + _cta(65536, 188, threads=128)),
+    ((7, 1, 20, 20), {}, 333, False, ("warp", 0, 42, 256), [(1, 42, 256, 64)] + _cta(333, 188, threads=128)),
+    ((7, 1, 20, 20), {}, 4096, True, ("lone_warp", 0, 4096, 32), _cta(4096, 188, threads=128)),
+    ((7, 1, 20, 20), {}, 4097, True, ("warp", 0, 513, 256), [(1, 513, 256, 64)] + _cta(4097, 188, threads=128)),
+    ((7, 1, 20, 20), {"n_sys": 333}, 333, True, ("lone_warp", 0, 333, 32), _cta(333, 188, threads=128)),
+    ((1, 1, 2, 2), {}, 5000, False, ("warp", 0, 625, 256), [(1, 625, 256, 8)]),
+    # tiles of 8 while the open instances fill the 132 SMs twice over (more than 2 112), then of 4 while they fill them with
+    # tiles of 2 (more than 528), then of 2
+    ((5, 2, 25, 25), {}, 2113, False, ("tile", 8, 265, 160), _cta(2113, 80, 232)),
+    ((5, 2, 25, 25), {}, 2112, True, ("tile", 4, 528, 160), _cta(2112, 80, 232)),
+    ((5, 2, 25, 25), {}, 529, True, ("tile", 4, 133, 160), _cta(529, 80, 232)),
+    ((5, 2, 25, 25), {}, 528, True, ("tile", 2, 264, 160), _cta(528, 80, 232)),
+    ((8, 4, 40, 40), {}, 16384, False, ("tile", 8, 2048, 352), _cta(16384, 80, 222)),
+    # shapes where tiles of 8 (or of 4) do not fit: the tile size never exceeds the largest that does
+    ((8, 4, 50, 50), {}, 100000, False, ("tile", 4, 25000, 416), _cta(100000, 80, 218)),
+    ((8, 4, 50, 50), {}, 528, True, ("tile", 2, 264, 416), _cta(528, 80, 218)),
+    ((8, 4, 83, 83), {}, 100000, False, ("tile", 2, 50000, 512), _cta(100000, 80, 204)),
+    # CTA team without tiles: per-instance systems, shapes beyond the tiles, a forced team size; rmax > 0 leaves one tier
+    ((5, 2, 25, 25), {"n_sys": 333}, 333, False, ("cta", 0, 333, 256), _cta(333, 80, 232)),
+    ((8, 4, 261, 261), {}, 5000, True, ("cta", 0, 5000, 256), _cta(5000, 96)),
+    ((7, 1, 20, 20), {"team_threads": 256, "rmax": 40}, 300, True, ("cta", 0, 300, 256), _cta(300, 40)),
+]
+
+
+def _bytes(shape, rmax=None):
+    """shared memory per instance of k_admm (rmax None) or of k_polish at capacity rmax"""
+    nx, nu, Np, Nc = shape
+    NX, NU = (Np + 1) * nx, Nc * nu
+    mc = NX + NU + (Nc + 1) * nu
+    if rmax is None:
+        return 8 * (4 * NU + NX + 2 * mc + nu + 8)
+    return 8 * (3 * NU + NX + 4 * mc + rmax * (rmax + 1) // 2 + rmax + nu + 2 + (mc + rmax + 3) // 2)
+
+
+@pytest.mark.parametrize("shape,opts,count,given,admm,tiers", ROUNDS,
+                         ids=[f"{'-'.join(map(str, s))}{''.join(f'-{k}{v}' for k, v in o.items())}-{c}{'-list' if g else ''}"
+                              for s, o, c, g, *_ in ROUNDS])
+def test_round_launch_at_h100(shape, opts, count, given, admm, tiers):
+    R = round_launch(*shape, count=count, list_given=given, **opts)
+    assert (R["admm"], R["tile_T"], R["admm_grid"], R["admm_threads"]) == admm
+    assert [(t["warp"], t["grid"], t["threads"], t["rmax"]) for t in R["tiers"]] == tiers
+    # shared memory: the kernels' per-instance carve-up (at the tier's capacity) times the instances per CTA
+    wpb = plan_launch(*shape, **opts)["wpb"]
+    assert R["admm_smem"] <= 232448 - 1024
+    if R["admm"] != "tile":
+        assert R["admm_smem"] == (wpb if R["admm"] == "warp" else 1) * _bytes(shape)
+    for t in R["tiers"]:
+        assert t["smem"] == (wpb if t["warp"] else 1) * _bytes(shape, t["rmax"])
+    assert launch_tiers(*shape, count=count, **opts)[int(given)] == tuple(c for *_, c in tiers)
 
 
 @pytest.mark.parametrize("shape", [(7, 1, 20, 20), (9, 1, 18, 10), (1, 2, 32, 32), (5, 2, 25, 25), (8, 4, 40, 40)])
