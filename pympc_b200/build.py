@@ -97,7 +97,8 @@ def tpm_shape_supported(nx, nu, Np, Nc=None):
 def jit_multi_input_shape(nx, nu, Np, Nc=None, Ad=None, Bd=None, verbose=False):
     """Build (once; cached under pympc_b200/_jit/) a copy of the library whose multi-input fast-path table holds the shape
     (nx, nu, Np, Nc) — with the sparsity pattern of (Ad, Bd) fixed at compile time when they are given and small enough for the
-    pattern masks (the sweeps then skip the structural zeros) — and return its path.  Raises on shapes outside
+    pattern masks (the sweeps then skip the structural zeros) — and return its path.  Per-instance systems (Ad of shape
+    (batch, nx, nx), Bd (batch, nx, nu)) compile the union of the instances' patterns.  Raises on shapes outside
     tpm_shape_supported."""
     import numpy as np
     Nc = Np if Nc is None else Nc
@@ -105,8 +106,8 @@ def jit_multi_input_shape(nx, nu, Np, Nc=None, Ad=None, Bd=None, verbose=False):
         raise ValueError(TPM_DOMAIN)
     line = f"BMPC_TPM_SHAPE({nx}, {nu}, {Np}, {Nc})"; tag = f"m{nx}_{nu}_{Np}_{Nc}"
     if Ad is not None and Bd is not None and nx * nx <= 64 and nx * nu <= 32:
-        A = np.asarray(Ad, float).reshape(nx, nx); Bm = np.asarray(Bd, float).reshape(nx, nu)
-        am = sum(1 << i for i, v in enumerate(A.ravel()) if v != 0.0); bm = sum(1 << i for i, v in enumerate(Bm.ravel()) if v != 0.0)
+        A = (np.asarray(Ad, float).reshape(-1, nx, nx) != 0.0).any(axis=0); Bm = (np.asarray(Bd, float).reshape(-1, nx, nu) != 0.0).any(axis=0)
+        am = sum(1 << i for i, v in enumerate(A.ravel()) if v); bm = sum(1 << i for i, v in enumerate(Bm.ravel()) if v)
         if am != (1 << (nx * nx)) - 1 or bm != (1 << (nx * nu)) - 1:
             line = f"BMPC_TPM_SPARSE_SHAPE({nx}, {nu}, {Np}, {Nc}, 0x{am:x}ull, 0x{bm:x}u)\n" + line      # the dense entry stays behind it
             tag += f"_{am:x}_{bm:x}"

@@ -922,7 +922,8 @@ __global__ void __launch_bounds__(TpiPolLayout<S>::warps * 32, 1) k_tpi_pol(cons
 
 
 // ------------------------------------------------------------------------------------------------
-// Multi-input fast path (bmpc_tpm.cuh): K5 of shapes with nu > 1 and one shared system — the constrained Riccati polish with one
+// Multi-input fast path (bmpc_tpm.cuh): K5 of shapes with nu > 1, one shared system or per-instance systems (PERINST: parameters
+// from each instance's view, TpmPolView) — the constrained Riccati polish with one
 // THREAD per instance and one warp (32 instances) per CTA.  Gain rows in global memory (per resident warp: slots x 32 lanes,
 // lane-interleaved), working sets in local memory, the system in the constant bank (kernel parameter).
 //  mode -1: warm first round of a solve: per instance, the stored working sets shifted one stage (record flag set: its last
@@ -935,16 +936,50 @@ struct TpmArgs {
     const int32_t* list; int count, mode, cap, reset;
     int32_t* counts; int32_t* next_list; double* u0_out; double* um1_solved;
     double* W; unsigned long long* rec; int rec_stride;               // record of instance i: Np code words, mumax, flag (rec_stride 64-bit words)
+    const double* pview; int pstride;                                  // per-instance parameter blocks (PERINST instantiation): base and field stride (= batch)
 };
 struct TpmDiscard { unsigned long long sink; };
 
-template <class S, bool TV, bool EX>
-__global__ void __launch_bounds__(32) k_tpm_pol(const __grid_constant__ TpmParams<S> P, BmpcInst I, TpmArgs A) {
+// the parameters k_tpm_pol's sweeps read: the kernel parameter (one shared system) or instance inst's view (per-instance systems)
+template <bool PERINST, class S>
+__device__ __forceinline__ decltype(auto) tpm_params_of(const TpmParams<S>& P, const TpmArgs& A, int inst) {
+    if constexpr (PERINST) return TpmPolView<S>(A.pview + inst, (size_t)A.pstride);
+    else return (P);
+}
+
+// per-instance parameter blocks of the multi-input fast path (TpmPolView).  tpm_fill reads only the raw inputs and scal: valid on a
+// block whose condensed part is stale (after bmpc_update_problem).  nondiag: raised when some instance's QDu is not diagonal
+template <class S>
+__global__ void k_tpm_fill_view(BmpcSysOff o, const double* __restrict__ sys, size_t sys_stride, int B, double* __restrict__ pg,
+                                unsigned long long* nondiag) {
+    const int inst = blockIdx.x * blockDim.x + threadIdx.x;
+    if (inst >= B) return;
+    TpmParams<S> P;
+    const bool diag = tpm_fill<S>(sys + (size_t)inst * sys_stride, o, P);
+    const double* src = (const double*)&P;
+    for (int f = 0; f < TpmPolView<S>::NF; f++) pg[(size_t)f * B + inst] = src[f];
+    if (!diag) *nondiag = 1ull;
+}
+
+// sparsity pattern of n new per-instance matrices of cnt <= 64 entries (batch-major, instance i's at src[i * cnt]): bit f of *word is
+// raised when entry f is non-zero in some instance (*word zeroed by the caller)
+__global__ void k_tpm_pattern(const double* __restrict__ src, int cnt, int n, unsigned long long* word) {
+    const int inst = blockIdx.x * blockDim.x + threadIdx.x;
+    unsigned long long m = 0ull;
+    if (inst < n)
+        for (int f = 0; f < cnt; f++) if (src[(size_t)inst * cnt + f] != 0.0) m |= 1ull << f;
+    for (int s = 16; s > 0; s >>= 1) m |= __shfl_xor_sync(0xffffffffu, m, s);
+    if ((threadIdx.x & 31) == 0 && m) atomicOr(word, m);
+}
+
+template <class S, bool TV, bool EX, bool PERINST>
+__global__ void __launch_bounds__(32) k_tpm_pol(const __grid_constant__ TpmParams<S> Pk, BmpcInst I, TpmArgs A) {
     using L = TpmLayout<S>; using CD = TpmCode<S>;
     constexpr int nx = S::nx, nu = S::nu, Np = S::Np, NU = S::NU, mc = S::mc, NX = S::NX;
     const int lane = threadIdx.x, idx = blockIdx.x * 32 + lane;
     const bool valid = idx < A.count;
     const int inst = valid ? (A.list ? A.list[idx] : idx) : 0;
+    auto&& P = tpm_params_of<PERINST>(Pk, A, inst);
     TpiStreamAcc W{A.W + (size_t)blockIdx.x * L::slots * 32 + lane, 32};
     uint64_t cur[Np], atb[Np];
     uint64_t dump = 0ull; uint64_t* const dp = &dump;
@@ -1044,6 +1079,8 @@ __global__ void __launch_bounds__(32) k_tpm_pol(const __grid_constant__ TpmParam
 struct TpmEntry {
     int nx, nu, Np, Nc; unsigned long long amask; unsigned bmask; size_t par_bytes; int slots;
     bool (*fill)(const double* hs, const BmpcSysOff& o, void* pp);
+    int view_fields; void (*fill_view)(struct bmpc_handle* h);
+    int view_ad, view_bd;              // field numbers of Ad and Bd in the per-instance parameter view (k_sys_refresh)
     void (*launch)(struct bmpc_handle* h, const int32_t* list, int count, int mode, int cap, int reset, int32_t* next_list, int exchange);
 };
 
@@ -1095,12 +1132,21 @@ struct bmpc_handle {
     bool pending = false;              // a round is in flight and has not been retired by the host yet
     int tpi_kind = 0;                  // 0 none, else 1 + index into g_tpi_table (compiled fast-path shapes)
     void *tpi_admm_params = nullptr, *tpi_polish_params = nullptr;   // host copies of the parameter blocks
-    double* tpi_view = nullptr;       // per-instance parameter blocks of the fast path (n_sys = batch), field-major
+    // the fast path's per-instance parameter blocks (n_sys = batch; TpiPolView or TpmPolView): field f of instance i at p[f * B + i].
+    // Recorded once at setup by whichever fast path owns it; bmpc_update_problem writes Ad / Bd into fields ad / bd (k_sys_refresh)
+    // and rebuilds the rest with fill
+    struct { double* p; int fields, ad, bd; void (*fill)(bmpc_handle* h); } view = {};
     bool codes_valid = false;         // the stored working sets come from a fast-path polish of the whole batch
     int tpm_kind = 0;                  // 0 none, else 1 + index into g_tpm_table (compiled multi-input fast-path shapes)
     void* tpm_params = nullptr;        // host copy of the parameter block
     double* tpm_W = nullptr; unsigned long long* tpm_rec = nullptr;   // gain rows of the resident warps, working-set records
     int tpm_W_slots = 0;               // gain slots per lane tpm_W was allocated for
+    // per-instance systems on the multi-input fast path (tpm_view_handle): the union of the instances' (Ad, Bd) patterns and whether
+    // some instance's QDu is not diagonal decide the entry (tpm_select_view).  tpm_word (device) / tpm_hword (pinned host): the
+    // pattern words of a device update [0] Ad, [1] Bd, and [2] the "QDu not diagonal" flag of k_tpm_fill_view
+    bool tpm_pi = false;
+    unsigned long long tpm_am = 0ull; unsigned tpm_bm = 0u; bool tpm_nondiag = false;
+    unsigned long long *tpm_word = nullptr, *tpm_hword = nullptr;
     BmpcPolicy policy = {};            // round policy of the chosen kernel family (bmpc_rounds.cuh)
     // time-varying (Ad, Bd), bmpc_update_system.  Per-instance systems: every instance's condensed block carries the generation it
     // was condensed for (sys_gen[i]); bmpc_update_system moves the handle's counter ahead of all of them and k_condense_list brings
@@ -1138,11 +1184,11 @@ static void launch_tpi_pol(bmpc_handle* h, const int32_t* list, int count, int m
     if (grid < 1) grid = 1;
     const size_t sm = L::smem;
     constexpr int threads = L::warps * 32;          // the kernel's last-warp exit count assumes exactly this block size
-    A.pview = h->tpi_view; A.pstride = h->cfg.batch;
+    A.pview = h->view.p; A.pstride = h->cfg.batch;
     A.host_counts = h->h_count; A.epoch = h->spin_epoch;
     A.gflags = h->gflags; A.gpeers = h->gpeers; A.g_npeer = h->g_npeer; A.g_rank = h->g_rank; A.g_world = h->g_world;
     A.g_epoch = (h->gflags && h->spin_epoch && h->g_world > 1) ? h->g_epoch : 0;
-    if (h->tpi_view) {
+    if (h->view.p) {
         if (h->xref_mode) k_tpi_pol<S, true, true><<<grid, threads, sm, h->stream>>>(PP, h->I, A);
         else k_tpi_pol<S, false, true><<<grid, threads, sm, h->stream>>>(PP, h->I, A);
     } else {
@@ -1178,7 +1224,7 @@ static void tpi_fill_entry(const double* hs, const BmpcSysOff& o, void* pa, void
 template <class S>
 static void tpi_fill_view_entry(bmpc_handle* h) {
     const int B = h->cfg.batch;
-    k_tpi_fill_view<S><<<(B + 63) / 64, 64, 0, h->stream>>>(h->o, h->sys, (size_t)h->o.total, B, h->tpi_view);
+    k_tpi_fill_view<S><<<(B + 63) / 64, 64, 0, h->stream>>>(h->o, h->sys, (size_t)h->o.total, B, h->view.p);
 }
 template <class S>
 static constexpr int tpi_view_field_ad() { using PS = TpiPolParams<S>; return (int)(offsetof(PS, Ad) / sizeof(double)); }
@@ -1218,21 +1264,42 @@ static void launch_tpm(bmpc_handle* h, const int32_t* list, int count, int mode,
     A.list = list; A.count = count; A.mode = mode; A.cap = cap; A.reset = reset;
     A.counts = h->counts + BMPC_CNT * h->cpar; A.next_list = next_list; A.u0_out = h->I.u0; A.um1_solved = h->um1_solved;
     A.W = h->tpm_W; A.rec = h->tpm_rec; A.rec_stride = S::Np + 2;
+    A.pview = h->view.p; A.pstride = h->cfg.batch;
     const TpmParams<S>& P = *(const TpmParams<S>*)h->tpm_params;
     const int grid = (count + 31) / 32;
-    // exchange: the straggler rounds' instantiation (hard rows change by single exchanges, tpm_forward<S, true>)
-    if (exchange) {
-        if (h->xref_mode) k_tpm_pol<S, true, true><<<grid, 32, 0, h->stream>>>(P, h->I, A);
-        else k_tpm_pol<S, false, true><<<grid, 32, 0, h->stream>>>(P, h->I, A);
+    // exchange: the straggler rounds' instantiation (hard rows change by single exchanges, tpm_forward<S, true>); per-instance
+    // systems (h->tpm_pi): the instantiation that reads each instance's view
+    if (h->tpm_pi) {
+        if (exchange) {
+            if (h->xref_mode) k_tpm_pol<S, true, true, true><<<grid, 32, 0, h->stream>>>(P, h->I, A);
+            else k_tpm_pol<S, false, true, true><<<grid, 32, 0, h->stream>>>(P, h->I, A);
+        } else {
+            if (h->xref_mode) k_tpm_pol<S, true, false, true><<<grid, 32, 0, h->stream>>>(P, h->I, A);
+            else k_tpm_pol<S, false, false, true><<<grid, 32, 0, h->stream>>>(P, h->I, A);
+        }
+    } else if (exchange) {
+        if (h->xref_mode) k_tpm_pol<S, true, true, false><<<grid, 32, 0, h->stream>>>(P, h->I, A);
+        else k_tpm_pol<S, false, true, false><<<grid, 32, 0, h->stream>>>(P, h->I, A);
     } else {
-        if (h->xref_mode) k_tpm_pol<S, true, false><<<grid, 32, 0, h->stream>>>(P, h->I, A);
-        else k_tpm_pol<S, false, false><<<grid, 32, 0, h->stream>>>(P, h->I, A);
+        if (h->xref_mode) k_tpm_pol<S, true, false, false><<<grid, 32, 0, h->stream>>>(P, h->I, A);
+        else k_tpm_pol<S, false, false, false><<<grid, 32, 0, h->stream>>>(P, h->I, A);
     }
     h->stats.launches++;
 }
 template <class S>
 static bool tpm_fill_entry(const double* hs, const BmpcSysOff& o, void* pp) { return tpm_fill<S>(hs, o, *(TpmParams<S>*)pp); }
-#define BMPC_TPM_ENTRY(S_) {S_::nx, S_::nu, S_::Np, S_::Nc, S_::amask, S_::bmask, sizeof(TpmParams<S_>), TpmLayout<S_>::slots, tpm_fill_entry<S_>, launch_tpm<S_>},
+template <class S>
+static void tpm_fill_view_entry(bmpc_handle* h) {
+    const int B = h->cfg.batch;
+    cudaMemsetAsync(h->tpm_word + 2, 0, sizeof(unsigned long long), h->stream);
+    k_tpm_fill_view<S><<<(B + 63) / 64, 64, 0, h->stream>>>(h->o, h->sys, (size_t)h->o.total, B, h->view.p, h->tpm_word + 2);
+}
+template <class S>
+static constexpr int tpm_view_field_ad() { using PS = TpmParams<S>; return (int)(offsetof(PS, Ad) / sizeof(double)); }
+template <class S>
+static constexpr int tpm_view_field_bd() { using PS = TpmParams<S>; return (int)(offsetof(PS, Bd) / sizeof(double)); }
+#define BMPC_TPM_ENTRY(S_) {S_::nx, S_::nu, S_::Np, S_::Nc, S_::amask, S_::bmask, sizeof(TpmParams<S_>), TpmLayout<S_>::slots, tpm_fill_entry<S_>, \
+                            TpmPolView<S_>::NF, tpm_fill_view_entry<S_>, tpm_view_field_ad<S_>(), tpm_view_field_bd<S_>(), launch_tpm<S_>},
 #define BMPC_TPM_SHAPE(NX_, NU_, NP_, NC_) BMPC_TPM_ENTRY(BMPC_TPM_T4(TpiShape, NX_, NU_, NP_, NC_))
 #define BMPC_TPM_SPARSE_SHAPE(NX_, NU_, NP_, NC_, AM_, BM_) BMPC_TPM_ENTRY(BMPC_TPM_T6(TpmSparseShape, NX_, NU_, NP_, NC_, AM_, BM_))
 #define BMPC_TPM_T4(T_, a, b, c, d) T_<a, b, c, d>
@@ -1409,7 +1476,9 @@ void bmpc_destroy(bmpc_handle* h) {
     for (void* p : ptrs) if (p) cudaFree(p);
     if (h->h_count) cudaFreeHost(h->h_count);
     free(h->tpi_admm_params); free(h->tpi_polish_params); free(h->tpm_params);
-    if (h->tpi_view) cudaFree(h->tpi_view);
+    if (h->view.p) cudaFree(h->view.p);
+    if (h->tpm_word) cudaFree(h->tpm_word);
+    if (h->tpm_hword) cudaFreeHost(h->tpm_hword);
     if (h->tpm_W) cudaFree(h->tpm_W);
     if (h->tpm_rec) cudaFree(h->tpm_rec);
     if (h->sys_gen) cudaFree(h->sys_gen);
@@ -1542,30 +1611,32 @@ static int check_condensed(bmpc_handle* h, const char* who) {
     return BMPC_OK;
 }
 
-// multi-input fast path: the first compiled entry of the shape whose (Ad, Bd) pattern masks contain the system's (blk: system block
-// on the host, inputs at their block offsets); 0: none
+// multi-input fast path: compiled shape, soft state rows, polish on (shared systems: bmpc_setup / derive_from_block; per-instance
+// systems: tpm_select_view)
 static bool tpm_eligible(const bmpc_handle* h) {
-    return h->cfg.fast_path && !h->tpi_kind && h->cfg.soft_on && h->cfg.n_sys <= 1 && h->cfg.polish;
+    return h->cfg.fast_path && !h->tpi_kind && h->cfg.soft_on && h->cfg.polish;
 }
-static int tpm_match(const bmpc_handle* h, const double* blk) {
-    const BmpcDims& d = h->d; const BmpcSysOff& o = h->o;
-    unsigned long long am = 0ull; unsigned bm = 0u;
-    if (d.nx * d.nx <= 64 && d.nx * d.nu <= 32) {
-        for (int i = 0; i < d.nx * d.nx; i++) if (blk[o.Ad + i] != 0.0) am |= 1ull << i;
-        for (int i = 0; i < d.nx * d.nu; i++) if (blk[o.Bd + i] != 0.0) bm |= 1u << i;
-    } else { am = ~0ull; bm = ~0u; }
+// the (Ad, Bd) sparsity pattern of n systems (system i's Ad at Ad[i * stride], Bd at Bd[i * stride]), as the union over them: bit
+// q nx + b of *am: Ad[q][b] non-zero in some system, bit a nu + j of *bm: Bd[a][j].  Shapes beyond the masks: all bits
+static void tpm_pattern(const BmpcDims& d, const double* Ad, const double* Bd, int n, size_t stride, unsigned long long* am, unsigned* bm) {
+    *am = 0ull; *bm = 0u;
+    if (d.nx * d.nx > 64 || d.nx * d.nu > 32) { *am = ~0ull; *bm = ~0u; return; }
+    for (int s = 0; s < n; s++) {
+        if (Ad) for (int i = 0; i < d.nx * d.nx; i++) if (Ad[s * stride + i] != 0.0) *am |= 1ull << i;
+        if (Bd) for (int i = 0; i < d.nx * d.nu; i++) if (Bd[s * stride + i] != 0.0) *bm |= 1u << i;
+    }
+}
+// the first compiled entry of the shape whose pattern masks contain the pattern (am, bm); 0: none
+static int tpm_match(const BmpcDims& d, unsigned long long am, unsigned bm) {
     for (int k = find_shape(g_tpm_table, g_tpm_count, d); k >= 0; k = find_shape(g_tpm_table, g_tpm_count, d, k + 1))
         if ((am & ~g_tpm_table[k].amask) == 0ull && (bm & ~g_tpm_table[k].bmask) == 0u) return k + 1;
     return 0;
 }
-// parameter block and workspace of multi-input entry `kind` from the condensed block hs (host copy); the entry stays off when its
-// fill declines (QDu not diagonal: team kernels).  fresh: the stored working-set records start empty (the next warm solve reads
+static bool tpm_sparse(int kind) { return kind && (~g_tpm_table[kind - 1].amask || ~g_tpm_table[kind - 1].bmask); }
+// gain rows and working-set records of multi-input entry `kind`.  fresh: the stored records start empty (the next warm solve reads
 // its working sets off v*)
-static int tpm_prepare(bmpc_handle* h, const double* hs, int kind, bool fresh) {
+static int tpm_alloc(bmpc_handle* h, int kind, bool fresh) {
     const TpmEntry& te = g_tpm_table[kind - 1];
-    free(h->tpm_params); h->tpm_params = malloc(te.par_bytes);
-    h->tpm_kind = te.fill(hs, h->o, h->tpm_params) ? kind : 0;
-    if (!h->tpm_kind) return BMPC_OK;
     const size_t B = h->cfg.batch, nwarp = (B + 31) / 32;
     if (h->tpm_W && h->tpm_W_slots < te.slots) { cudaFree(h->tpm_W); h->tpm_W = nullptr; }
     if (!h->tpm_W) { BMPC_CUDA(cudaMalloc((void**)&h->tpm_W, sizeof(double) * nwarp * 32 * (size_t)te.slots)); h->tpm_W_slots = te.slots; }
@@ -1575,23 +1646,48 @@ static int tpm_prepare(bmpc_handle* h, const double* hs, int kind, bool fresh) {
 }
 
 static int policy_family(const bmpc_handle* h) {
-    return h->tpi_kind ? (h->tpi_view ? BMPC_FAM_TPI_VIEW : BMPC_FAM_TPI) : h->tpm_kind ? BMPC_FAM_TPM : BMPC_FAM_TEAM;
+    return h->tpi_kind ? (h->view.p ? BMPC_FAM_TPI_VIEW : BMPC_FAM_TPI) : h->tpm_kind ? BMPC_FAM_TPM : BMPC_FAM_TEAM;
 }
 
 // what the host derives from system 0's condensed block (bmpc_setup; bmpc_update_problem on a shared system): the single-input fast
 // path's constant-bank parameters, the multi-input entry and the kernel family.  Reads the block back only when a fast path is in play
-// (the single-input one, or multi-input entries of this shape: their pattern match reads Ad, Bd).  fresh: empty multi-input records
+// (the single-input one, or multi-input entries of this shape: their pattern match reads Ad, Bd).  fresh: empty multi-input records.
+// The multi-input entry stays off when its fill declines (QDu not diagonal: team kernels).  (Per-instance systems: tpm_select_view)
 static int derive_from_block(bmpc_handle* h, bool fresh) {
     const int old = h->tpm_kind;
-    const bool tpm = tpm_eligible(h) && find_shape(g_tpm_table, g_tpm_count, h->d) >= 0;
+    const bool tpm = tpm_eligible(h) && h->cfg.n_sys <= 1 && find_shape(g_tpm_table, g_tpm_count, h->d) >= 0;
     h->tpm_kind = 0;
     if (h->tpi_kind || tpm) {
         std::vector<double> hs(h->o.total);
         BMPC_CUDA(cudaMemcpyAsync(hs.data(), h->sys, sizeof(double) * h->o.total, cudaMemcpyDeviceToHost, h->stream));
         BMPC_CUDA(cudaStreamSynchronize(h->stream));
         if (h->tpi_kind) g_tpi_table[h->tpi_kind - 1].fill(hs.data(), h->o, h->tpi_admm_params, h->tpi_polish_params);
-        const int tk = tpm ? tpm_match(h, hs.data()) : 0;
-        if (tk) { int rc = tpm_prepare(h, hs.data(), tk, fresh || tk != old); if (rc) return rc; }
+        unsigned long long am; unsigned bm;
+        tpm_pattern(h->d, hs.data() + h->o.Ad, hs.data() + h->o.Bd, 1, 0, &am, &bm);
+        const int tk = tpm ? tpm_match(h->d, am, bm) : 0;
+        if (tk) {
+            free(h->tpm_params); h->tpm_params = malloc(g_tpm_table[tk - 1].par_bytes);
+            if (g_tpm_table[tk - 1].fill(hs.data(), h->o, h->tpm_params)) {
+                h->tpm_kind = tk;
+                int rc = tpm_alloc(h, tk, fresh || tk != old); if (rc) return rc;
+            }
+        }
+    }
+    h->policy.family = policy_family(h);
+    return BMPC_OK;
+}
+
+// per-instance systems on the multi-input fast path: the entry whose masks contain the union of the instances' patterns (tpm_am,
+// tpm_bm), none while some instance's QDu is not diagonal (team kernels).  The view itself is kept current by the caller (setup and
+// every update fill it, whichever family runs), so a change of entry needs only the workspace; it starts with empty records, as after
+// setup (fresh).
+static int tpm_select_view(bmpc_handle* h, bool fresh) {
+    const int old = h->tpm_kind;
+    const int kind = h->tpm_nondiag ? 0 : tpm_match(h->d, h->tpm_am, h->tpm_bm);
+    h->tpm_kind = kind;
+    if (kind) {
+        if (!h->tpm_params) h->tpm_params = calloc(1, g_tpm_table[kind - 1].par_bytes);     // (k_tpm_pol<..., PERINST> reads the view)
+        int rc = tpm_alloc(h, kind, fresh || kind != old); if (rc) return rc;
     }
     h->policy.family = policy_family(h);
     return BMPC_OK;
@@ -1635,18 +1731,40 @@ int bmpc_setup(bmpc_handle* h, const double* Ad, const double* Bd, const double*
         free(h->tpi_admm_params); free(h->tpi_polish_params);
         h->tpi_admm_params = malloc(te.admm_bytes); h->tpi_polish_params = malloc(te.ric_bytes);
         if (te.configure()) { h->err = "fast path: shared-memory configuration failed"; return BMPC_ERR_CUDA; }
-        if (h->tpi_view) { cudaFree(h->tpi_view); h->tpi_view = nullptr; }
+        if (h->view.p) { cudaFree(h->view.p); h->view = {}; }
         if (ns > 1) {
             // one parameter block per instance, built on the device from each instance's condensed system block
-            BMPC_CUDA(cudaMalloc((void**)&h->tpi_view, sizeof(double) * (size_t)te.view_fields * h->cfg.batch));
+            BMPC_CUDA(cudaMalloc((void**)&h->view.p, sizeof(double) * (size_t)te.view_fields * h->cfg.batch));
+            h->view.fields = te.view_fields; h->view.ad = te.view_ad; h->view.bd = te.view_bd; h->view.fill = te.fill_view;
             te.fill_view(h);
             BMPC_CUDA(cudaGetLastError());
         }
     }
-    // the fast paths' parameters and the kernel family; multi-input fast path: compiled shape, one shared system, soft state rows,
-    // diagonal QDu (sparsity pattern of (Ad, Bd): an entry fits when its compile-time masks contain it)
+    // the fast paths' parameters and the kernel family; multi-input fast path: compiled shape, soft state rows, diagonal QDu
+    // (sparsity pattern of (Ad, Bd): an entry fits when its compile-time masks contain it)
     int rc = derive_from_block(h, true);
     if (rc) return rc;
+    // per-instance systems on the multi-input fast path: the view is kept whichever family runs (a later update may bring the
+    // handle onto an entry); the entry matches the union of the instances' patterns, and every QDu must be diagonal
+    const int tpm_shape = find_shape(g_tpm_table, g_tpm_count, d);
+    h->tpm_pi = ns > 1 && tpm_eligible(h) && tpm_shape >= 0;
+    if (h->tpm_pi) {
+        const TpmEntry& te = g_tpm_table[tpm_shape];
+        if (!h->tpm_word) BMPC_CUDA(cudaMalloc((void**)&h->tpm_word, 3 * sizeof(unsigned long long)));
+        if (!h->tpm_hword) BMPC_CUDA(cudaMallocHost((void**)&h->tpm_hword, 3 * sizeof(unsigned long long)));
+        if (!h->view.p) BMPC_CUDA(cudaMalloc((void**)&h->view.p, sizeof(double) * (size_t)te.view_fields * h->cfg.batch));
+        h->view.fields = te.view_fields; h->view.ad = te.view_ad; h->view.bd = te.view_bd; h->view.fill = te.fill_view;
+        te.fill_view(h);
+        BMPC_CUDA(cudaGetLastError());
+        tpm_pattern(d, in.data() + P[0].off, in.data() + P[1].off, ns, o.pw, &h->tpm_am, &h->tpm_bm);
+        h->tpm_nondiag = false;
+        for (int si = 0; si < ns; si++) {
+            const double* q = in.data() + (size_t)si * o.pw + P[5].off;
+            for (int i = 0; i < d.nu * d.nu; i++) if (i / d.nu != i % d.nu && q[i] != 0.0) h->tpm_nondiag = true;
+        }
+        rc = tpm_select_view(h, true);
+        if (rc) return rc;
+    }
     const bmpc_config& c = h->cfg;
     h->policy = bmpc_make_policy(h->policy.family, c.polish, c.first_iters, c.cold_iters, c.max_iter, c.pdas_steps, c.shift_warm);
     // time-varying problem data on per-instance systems: when the weights keep H positive definite for ANY (Ad, Bd),
@@ -1726,10 +1844,10 @@ int bmpc_update_problem(bmpc_handle* h, const double* Ad, const double* Bd, cons
     // per-instance systems: the new arrays go into every block and into the fast path's parameter view; the condense is deferred
     // to the launches that read a condensed block (condense_stale) — unless H may lose definiteness, then all of it now + the check
     const int B = h->cfg.batch;
-    const TpiEntry* te = h->tpi_kind ? &g_tpi_table[h->tpi_kind - 1] : nullptr;
+    const bool hv = h->view.p != nullptr;                // the handle's parameter view (either fast path)
     if (!on_device && !h->sys_stage) BMPC_CUDA(cudaMalloc((void**)&h->sys_stage, sizeof(double) * (size_t)B * o.pw));
     BmpcRefreshTab T = {}; size_t per = 0;
-    bool view_fill = false;                              // an array the view holds only through derived fields (k_tpi_fill_view)
+    bool view_fill = false;                              // an array the view holds only through derived fields (view.fill)
     for (int f = 0; f < 13; f++) {
         if (!src[f]) continue;
         const double* s = src[f];
@@ -1737,16 +1855,46 @@ int bmpc_update_problem(bmpc_handle* h, const double* Ad, const double* Bd, cons
             BMPC_CUDA(cudaMemcpyAsync(h->sys_stage + (size_t)B * P[f].off, s, sizeof(double) * B * P[f].cnt, cudaMemcpyHostToDevice, h->stream));
             s = h->sys_stage + (size_t)B * P[f].off;
         }
-        const int view = !te ? -1 : f == 0 ? te->view_ad : f == 1 ? te->view_bd : -1;
-        view_fill = view_fill || (te && f >= 2);
+        const int view = !hv ? -1 : f == 0 ? h->view.ad : f == 1 ? h->view.bd : -1;
+        view_fill = view_fill || (hv && f >= 2);
         T.seg[T.n++] = BmpcRefreshSeg{s, P[f].off, P[f].cnt, view};
         per += (size_t)P[f].cnt;
     }
     const size_t n = (size_t)B * per;
-    k_sys_refresh<<<(unsigned)((n + 255) / 256), 256, 0, h->stream>>>(h->sys, h->I.sys_stride, B, T, h->tpi_view);
+    k_sys_refresh<<<(unsigned)((n + 255) / 256), 256, 0, h->stream>>>(h->sys, h->I.sys_stride, B, T, h->view.p);
     BMPC_CUDA(cudaGetLastError());
-    if (view_fill) { te->fill_view(h); BMPC_CUDA(cudaGetLastError()); }
+    if (view_fill) { h->view.fill(h); BMPC_CUDA(cudaGetLastError()); }
     h->sys_gen_cur++; h->sys_stale = true;
+    // multi-input fast path on per-instance systems: the union pattern of the new (Ad, Bd) and "QDu not diagonal" decide the entry
+    // below.  Host arrays: decided here.  Device (Ad, Bd) on a sparse entry: k_tpm_pattern + one synchronising read of the pattern
+    // words; on the dense entry or the team kernels the pattern is taken as dense (nothing is read back).  Device QDu: the flag
+    // k_tpm_fill_view raised, read in the synchronisation of the definiteness check below
+    const bool qdu_dev = h->tpm_pi && QDu && on_device;
+    if (h->tpm_pi && model) {
+        if (!on_device) {
+            unsigned long long am; unsigned bm;
+            if (Ad) { tpm_pattern(d, Ad, nullptr, B, (size_t)P[0].cnt, &am, &bm); h->tpm_am = am; }
+            if (Bd) { tpm_pattern(d, nullptr, Bd, B, (size_t)P[1].cnt, &am, &bm); h->tpm_bm = bm; }
+        } else if (tpm_sparse(h->tpm_kind)) {
+            BMPC_CUDA(cudaMemsetAsync(h->tpm_word, 0, 2 * sizeof(unsigned long long), h->stream));
+            if (Ad) k_tpm_pattern<<<(B + 127) / 128, 128, 0, h->stream>>>(Ad, P[0].cnt, B, h->tpm_word);
+            if (Bd) k_tpm_pattern<<<(B + 127) / 128, 128, 0, h->stream>>>(Bd, P[1].cnt, B, h->tpm_word + 1);
+            BMPC_CUDA(cudaGetLastError());
+            BMPC_CUDA(cudaMemcpyAsync(h->tpm_hword, h->tpm_word, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
+            BMPC_CUDA(cudaStreamSynchronize(h->stream));
+            if (Ad) h->tpm_am = h->tpm_hword[0];
+            if (Bd) h->tpm_bm = (unsigned)h->tpm_hword[1];
+        } else {
+            if (Ad) h->tpm_am = ~0ull;
+            if (Bd) h->tpm_bm = ~0u;
+        }
+    }
+    if (h->tpm_pi && QDu && !on_device) {
+        h->tpm_nondiag = false;
+        for (int si = 0; si < B; si++)
+            for (int i = 0; i < d.nu * d.nu; i++) if (i / d.nu != i % d.nu && QDu[(size_t)si * d.nu * d.nu + i] != 0.0) h->tpm_nondiag = true;
+    }
+    if (qdu_dev) BMPC_CUDA(cudaMemcpyAsync(h->tpm_hword + 2, h->tpm_word + 2, sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
     // definiteness depends on the weights alone: new host weights decide the deferral again (every instance, with the arrays this
     // call kept: read back from the blocks); device weights are condensed and checked at once
     bool check = model && !h->sys_lazy;
@@ -1764,8 +1912,10 @@ int bmpc_update_problem(bmpc_handle* h, const double* Ad, const double* Bd, cons
         condense_stale(h, nullptr, B, nullptr);
         BMPC_CUDA(cudaGetLastError());
         int rc = check_condensed(h, "bmpc_update_problem");
-        if (rc) return rc;
+        if (qdu_dev) h->tpm_nondiag = h->tpm_hword[2] != 0ull;        // (check_condensed synchronised the stream)
+        if (rc) { if (h->tpm_pi) tpm_select_view(h, false); return rc; }   // refused; the entry still follows the arrays the blocks hold
     }
+    if (h->tpm_pi) { int rc = tpm_select_view(h, false); if (rc) return rc; }
     // (bounds and uref alone leave definiteness as it was: a handle refused after a failed update stays refused)
     if (check || h->sys_lazy) h->sys_bad = false;
     return BMPC_OK;
@@ -1832,9 +1982,10 @@ static int enqueue_round(bmpc_handle* h, const BmpcRoundPlan& p) {
             BMPC_CUDA(cudaMemcpyAsync(h->um1_solved, h->um1_cur, sizeof(double) * (size_t)B * h->d.nu, cudaMemcpyDefault, h->stream));   // (um1_cur may be mapped host memory)
         }
         BMPC_CUDA(cudaMemsetAsync(h->counts, 0, sizeof(int32_t) * 2 * BMPC_CNT, h->stream));     // this round's half and the next one's
-        // every launch below reads the condensed blocks of exactly this round's instances (per-instance systems after
-        // bmpc_update_system: bring them up to date first; the fast-path round above reads only the parameter view)
-        h->stats.launches += condense_stale(h, st.list, st.count, cnt + BMPC_CNT_COND);
+        // every team launch below reads the condensed blocks of exactly this round's instances (per-instance systems after
+        // bmpc_update_system: bring them up to date first).  The fast-path rounds without team ADMM (k_tpi_pol, k_tpm_pol alone)
+        // read only the parameters or the view, so a warm step they finish condenses nothing
+        if (team) h->stats.launches += condense_stale(h, st.list, st.count, cnt + BMPC_CNT_COND);
     }
     h->spin_epoch = 0;
     if (p.admm == BMPC_ADMM_NONE && p.polish == BMPC_POL_TPI) { h->epoch = (h->epoch % 1000000000) + 1; h->spin_epoch = h->epoch; ((volatile int32_t*)h->h_count)[BMPC_CNT_EPOCH] = 0; }

@@ -573,9 +573,13 @@ BMPC_HD int tpm_vstar_row(int k, int p) {
     return (i >= 1) ? NX + NU + nu + i - 1 : -1;
 }
 
+// The parameters of one system; returns "QDu diagonal" (the sweeps need it).  Reads only the system's inputs (Ad .. uref) and
+// scal[RHO], scal[RHOE], never the condensed arrays: the rows' bounds are the raw bounds (lo0 / hi0 copy them, periodic in nu) and a
+// row's rho follows the condense's rule (bmpc_row_rho).  So the fill stays valid on a block whose condensed part predates its inputs
+// (per-instance systems after bmpc_update_problem, k_tpm_fill_view) and gives bit for bit what a fill of the freshly condensed block gives.
 template <class S>
 BMPC_HOSTDEV bool tpm_fill(const double* sys, const BmpcSysOff& o, TpmParams<S>& P) {
-    constexpr int nx = S::nx, nu = S::nu, NU = S::NU, NX = S::NX;
+    constexpr int nx = S::nx, nu = S::nu;
     bool diag = true;
     for (int i = 0; i < nx * nx; i++) { P.Ad[i] = sys[o.Ad + i]; P.Qx[i] = sys[o.Qx + i]; P.QxN[i] = sys[o.QxN + i]; }
     for (int i = 0; i < nx * nu; i++) P.Bd[i] = sys[o.Bd + i];
@@ -585,13 +589,13 @@ BMPC_HOSTDEV bool tpm_fill(const double* sys, const BmpcSysOff& o, TpmParams<S>&
         P.QDu[i] = sys[o.QDu + i * nu + i];
         double q = 0.0; for (int j = 0; j < nu; j++) q += sys[o.Qu + i * nu + j] * sys[o.uref + j]; P.quref[i] = q;
     }
-    const double rho_e = sys[o.scal + BMPC_S_RHOE];
+    const double rho_e = sys[o.scal + BMPC_S_RHOE], rho = sys[o.scal + BMPC_S_RHO];
     auto tol = [](double b, double rel, double sgn) { return (fabs(b) > 1e300) ? b : b + sgn * rel * (1.0 + fabs(b)); };
     const double inf = 1.0 / 0.0;
     for (int a = 0; a < nx; a++) {
-        const double lo = sys[o.lo0 + nx + a], hi = sys[o.hi0 + nx + a];
+        const double lo = sys[o.xmin + a], hi = sys[o.xmax + a];          // the state rows of stage 1 (condensed rows nx + a)
         P.xlo[a] = lo; P.xhi[a] = hi; P.xlo_m[a] = tol(lo, 1e-11, -1.0); P.xhi_p[a] = tol(hi, 1e-11, 1.0);
-        const double xlo_p = tol(lo, 1e-11, 1.0), xhi_m = tol(hi, 1e-11, -1.0), cx = rho_e / sys[o.rho + nx + a];
+        const double xlo_p = tol(lo, 1e-11, 1.0), xhi_m = tol(hi, 1e-11, -1.0), cx = rho_e / bmpc_row_rho(lo, hi, rho);
         const double al[4] = {P.xlo_m[a], xhi_m, -inf, -inf}, ah[4] = {P.xhi_p[a], inf, xlo_p, inf};
         const double m[4] = {0.0, rho_e, rho_e, 0.0}, bd[4] = {0.0, hi, lo, 0.0};
         for (int l = 0; l < 4; l++) {
@@ -601,13 +605,45 @@ BMPC_HOSTDEV bool tpm_fill(const double* sys, const BmpcSysOff& o, TpmParams<S>&
     }
     for (int j = 0; j < nu; j++) {
         const int jc = (j + nu - 1) % nu;                               // channel whose bounds the chain row ending at j carries
-        P.ulo[j] = sys[o.lo0 + NX + j]; P.uhi[j] = sys[o.hi0 + NX + j];
-        P.flo[j] = sys[o.lo0 + NX + NU + j]; P.fhi[j] = sys[o.hi0 + NX + NU + j];
-        P.clo[j] = sys[o.lo0 + NX + NU + jc]; P.chi[j] = sys[o.hi0 + NX + NU + jc];      // lo0 / hi0 are periodic in nu over the block
+        P.ulo[j] = sys[o.umin + j]; P.uhi[j] = sys[o.umax + j];        // input row (condensed row NX + j)
+        P.flo[j] = sys[o.Dumin + j]; P.fhi[j] = sys[o.Dumax + j];      // first-block row (NX + NU + j)
+        P.clo[j] = sys[o.Dumin + jc]; P.chi[j] = sys[o.Dumax + jc];    // chain row (NX + NU + nu + jc)
         P.ulo_m[j] = tol(P.ulo[j], 1e-9, -1.0); P.uhi_p[j] = tol(P.uhi[j], 1e-9, 1.0);
         P.flo_m[j] = tol(P.flo[j], 1e-9, -1.0); P.fhi_p[j] = tol(P.fhi[j], 1e-9, 1.0);
         P.clo_m[j] = tol(P.clo[j], 1e-9, -1.0); P.chi_p[j] = tol(P.chi[j], 1e-9, 1.0);
-        P.irhou[j] = 1.0 / sys[o.rho + NX + j]; P.irhof[j] = 1.0 / sys[o.rho + NX + NU + j]; P.irhoc[j] = 1.0 / sys[o.rho + NX + NU + nu + jc];
+        P.irhou[j] = 1.0 / bmpc_row_rho(P.ulo[j], P.uhi[j], rho); P.irhof[j] = 1.0 / bmpc_row_rho(P.flo[j], P.fhi[j], rho);
+        P.irhoc[j] = 1.0 / bmpc_row_rho(P.clo[j], P.chi[j], rho);
     }
     return diag;
 }
+
+// ------------------------------------------------------------------------------------------------
+// Per-instance systems (n_sys = batch) on the multi-input fast path: one TpmParams<S> per instance in GLOBAL memory, field-major —
+// double number f of instance i at pg[f * B + i] — so that a warp's 32 consecutive instances read a field with one coalesced access.
+// TpmPolView offers the member names of TpmParams (P.Ad[i], P.xm[a][lab], P.ulo_m[j], ...), so the sweeps above compile unchanged
+// against either.  Unlike TpiPolView it keeps no pointer per field: every field is addressed from the one base pointer and the
+// stride, at an offset fixed at compile time (k_tpm_pol runs at the register limit; 30 field pointers would not fit beside it).
+template <int OFF>
+struct TpmVF { const double* p; size_t B; BMPC_HD double operator[](int i) const { return TpiGArr{p + (size_t)OFF * B, B}[i]; } };
+template <int OFF>
+struct TpmVF2 { const double* p; size_t B; BMPC_HD TpiGArr operator[](int a) const { return TpiGArr2{p + (size_t)OFF * B, B}[a]; } };
+template <class S>
+struct TpmPolView {
+    using PS = TpmParams<S>;
+    static constexpr int NF = (int)(sizeof(PS) / sizeof(double));
+#define BMPC_TVF(m) TpmVF<(int)(offsetof(PS, m) / sizeof(double))> m
+#define BMPC_TVF2(m) TpmVF2<(int)(offsetof(PS, m) / sizeof(double))> m
+    BMPC_TVF(Ad); BMPC_TVF(Bd); BMPC_TVF(Qx); BMPC_TVF(QxN); BMPC_TVF(Qu); BMPC_TVF(QDu); BMPC_TVF(quref);
+    BMPC_TVF(xlo); BMPC_TVF(xhi); BMPC_TVF(xlo_m); BMPC_TVF(xhi_p);
+    BMPC_TVF2(xacc_lo); BMPC_TVF2(xacc_hi); BMPC_TVF2(xm); BMPC_TVF2(xmb); BMPC_TVF2(xcm); BMPC_TVF2(xbnd);
+    BMPC_TVF(ulo); BMPC_TVF(uhi); BMPC_TVF(ulo_m); BMPC_TVF(uhi_p); BMPC_TVF(irhou);
+    BMPC_TVF(flo); BMPC_TVF(fhi); BMPC_TVF(flo_m); BMPC_TVF(fhi_p); BMPC_TVF(irhof);
+    BMPC_TVF(clo); BMPC_TVF(chi); BMPC_TVF(clo_m); BMPC_TVF(chi_p); BMPC_TVF(irhoc);
+#undef BMPC_TVF
+#undef BMPC_TVF2
+    BMPC_HD TpmPolView(const double* p, size_t B)
+        : Ad{p, B}, Bd{p, B}, Qx{p, B}, QxN{p, B}, Qu{p, B}, QDu{p, B}, quref{p, B}, xlo{p, B}, xhi{p, B}, xlo_m{p, B}, xhi_p{p, B},
+          xacc_lo{p, B}, xacc_hi{p, B}, xm{p, B}, xmb{p, B}, xcm{p, B}, xbnd{p, B},
+          ulo{p, B}, uhi{p, B}, ulo_m{p, B}, uhi_p{p, B}, irhou{p, B}, flo{p, B}, fhi{p, B}, flo_m{p, B}, fhi_p{p, B}, irhof{p, B},
+          clo{p, B}, chi{p, B}, clo_m{p, B}, chi_p{p, B}, irhoc{p, B} {}
+};

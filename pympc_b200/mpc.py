@@ -364,7 +364,8 @@ class MPCController:
         """The in-tree build, or — for a single-input shape its fast-path table does not hold — a per-shape build made on the spot
         (pympc_b200.build.jit_shape, cached): every (nx, 1, Np, Nc) runs on the thread-per-instance kernels, like the reference
         handles every shape uniformly (mpc.py:456-615).  Falls back to the generic team kernels with a warning if that build is
-        not possible (no nvcc on this machine)."""
+        not possible (no nvcc available).  With fast_path=2 a multi-input shape missing from the in-tree table is built the same
+        way (build.jit_multi_input_shape), per-instance multi-input systems included (the union of the instances' patterns)."""
         from . import build
         L = _lib.load()
         opts = self.solver_options
@@ -372,7 +373,10 @@ class MPCController:
         NX, NU = (self.Np + 1) * self.nx, self.Nc * self.nu
         small = (NX + NU + (self.Nc + 1) * self.nu) <= 192 and NU <= 64          # the library's own rule for the warp-team family
         tpi_fits = small and build.tpi_shape_supported(self.nx, self.nu, self.Np, self.Nc)    # the single-input kernels hold this shape
-        if wants_fast and int(opts.get("fast_path", 1)) >= 2 and not tpi_fits and build.tpm_shape_supported(self.nx, self.nu, self.Np, self.Nc) \
+        # per-instance systems (3-D Ad) with several inputs take the multi-input fast path too (the union of the instances' patterns)
+        wants_tpm = wants_fast or (self._per_instance and self.nu > 1 and opts.get("fast_path", 1) and not opts.get("team_threads", 0)
+                                   and opts.get("polish", 1) and self.SOFT_ON)
+        if wants_tpm and int(opts.get("fast_path", 1)) >= 2 and not tpi_fits and build.tpm_shape_supported(self.nx, self.nu, self.Np, self.Nc) \
                 and not L.bmpc_has_multi_input_fast_path(self.nx, self.nu, self.Np, self.Nc) and not os.environ.get("BMPC_NO_JIT"):
             # fast_path=2: also build the multi-input Riccati polish for this shape (and this system's sparsity pattern) on the spot
             try:
