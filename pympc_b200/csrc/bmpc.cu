@@ -190,7 +190,7 @@ struct BmpcRefreshTab { BmpcRefreshSeg seg[13]; int n; };
 // every instance's system block and the view-held ones into the view as well.  The condensed part of the block is NOT touched here:
 // the handle's generation counter has moved past every instance's stamp, and k_condense_list re-condenses an instance before the
 // first launch that reads its condensed block.  (The view's fields derived from bounds, weights or uref are rebuilt from the raw
-// fields by k_tpi_fill_view.)
+// fields by k_fill_view.)
 __global__ void k_sys_refresh(double* __restrict__ sys, size_t sys_stride, int B, const __grid_constant__ BmpcRefreshTab T,
                               double* __restrict__ view) {
     const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -820,16 +820,25 @@ __device__ __forceinline__ void tpi_pol_batch(const PP& P, const BmpcInst& I, co
     __syncwarp();
 }
 
-// per-instance parameter blocks (n_sys = batch): field-major in global memory, see TpiPolView.  tpi_fill_pol reads only the raw
-// inputs and scal: valid on a block whose condensed part is stale (after bmpc_update_problem)
+// the parameters of one system that a fast path's per-instance view holds; false: QDu is not diagonal (the multi-input sweeps need
+// it diagonal).  Both fills read only the raw inputs and scal: valid on a block whose condensed part is stale (after bmpc_update_problem)
 template <class S>
-__global__ void k_tpi_fill_view(BmpcSysOff o, const double* __restrict__ sys, size_t sys_stride, int B, double* __restrict__ pg) {
+__device__ __forceinline__ bool fill_view_params(const double* sys, const BmpcSysOff& o, TpiPolParams<S>& P) { tpi_fill_pol<S>(sys, o, P); return true; }
+template <class S>
+__device__ __forceinline__ bool fill_view_params(const double* sys, const BmpcSysOff& o, TpmParams<S>& P) { return tpm_fill<S>(sys, o, P); }
+
+// per-instance parameter blocks (n_sys = batch) of either fast path, field-major in global memory (TpiPolView, TpmPolView): field f
+// of instance i at pg[f * B + i].  nondiag: raised when some instance's QDu is not diagonal (never by the single-input fill)
+template <class PS>
+__global__ void k_fill_view(BmpcSysOff o, const double* __restrict__ sys, size_t sys_stride, int B, double* __restrict__ pg,
+                            unsigned long long* nondiag) {
     const int inst = blockIdx.x * blockDim.x + threadIdx.x;
     if (inst >= B) return;
-    TpiPolParams<S> P;
-    tpi_fill_pol<S>(sys + (size_t)inst * sys_stride, o, P);
+    PS P;
+    const bool diag = fill_view_params(sys + (size_t)inst * sys_stride, o, P);
     const double* src = (const double*)&P;
-    for (int f = 0; f < TpiPolView<S>::NF; f++) pg[(size_t)f * B + inst] = src[f];
+    for (int f = 0; f < (int)(sizeof(PS) / sizeof(double)); f++) pg[(size_t)f * B + inst] = src[f];
+    if (!diag) *nondiag = 1ull;
 }
 
 template <class S, bool TV, bool PERINST>
@@ -947,20 +956,6 @@ __device__ __forceinline__ decltype(auto) tpm_params_of(const TpmParams<S>& P, c
     else return (P);
 }
 
-// per-instance parameter blocks of the multi-input fast path (TpmPolView).  tpm_fill reads only the raw inputs and scal: valid on a
-// block whose condensed part is stale (after bmpc_update_problem).  nondiag: raised when some instance's QDu is not diagonal
-template <class S>
-__global__ void k_tpm_fill_view(BmpcSysOff o, const double* __restrict__ sys, size_t sys_stride, int B, double* __restrict__ pg,
-                                unsigned long long* nondiag) {
-    const int inst = blockIdx.x * blockDim.x + threadIdx.x;
-    if (inst >= B) return;
-    TpmParams<S> P;
-    const bool diag = tpm_fill<S>(sys + (size_t)inst * sys_stride, o, P);
-    const double* src = (const double*)&P;
-    for (int f = 0; f < TpmPolView<S>::NF; f++) pg[(size_t)f * B + inst] = src[f];
-    if (!diag) *nondiag = 1ull;
-}
-
 // sparsity pattern of n new per-instance matrices of cnt <= 64 entries (batch-major, instance i's at src[i * cnt]): bit f of *word is
 // raised when entry f is non-zero in some instance (*word zeroed by the caller)
 __global__ void k_tpm_pattern(const double* __restrict__ src, int cnt, int n, unsigned long long* word) {
@@ -1075,24 +1070,18 @@ __global__ void __launch_bounds__(32) k_tpm_pol(const __grid_constant__ TpmParam
     }
 }
 
-// Compiled multi-input fast-path shapes: one line per shape in csrc/tpm_shapes.inc
-struct TpmEntry {
-    int nx, nu, Np, Nc; unsigned long long amask; unsigned bmask; size_t par_bytes; int slots;
-    bool (*fill)(const double* hs, const BmpcSysOff& o, void* pp);
-    int view_fields; void (*fill_view)(struct bmpc_handle* h);
-    int view_ad, view_bd;              // field numbers of Ad and Bd in the per-instance parameter view (k_sys_refresh)
-    void (*launch)(struct bmpc_handle* h, const int32_t* list, int count, int mode, int cap, int reset, int32_t* next_list, int exchange);
-};
-
-// Compiled fast-path shapes (nx, nu, Np, Nc) with nu == 1 and Nc == Np: one line per shape in csrc/tpi_shapes.inc
-// (`python -m pympc_b200.build --add-shape nx,1,Np` appends one and rebuilds).
-struct TpiEntry {
+// One compiled fast-path entry: a shape of the single-input fast path (one line of csrc/tpi_shapes.inc; `python -m pympc_b200.build
+// --add-shape nx,1,Np` appends one and rebuilds) or a shape and (Ad, Bd) pattern of the multi-input one (csrc/tpm_shapes.inc)
+struct BmpcFastEntry {
+    int family;                        // BMPC_FAM_TPI or BMPC_FAM_TPM
     int nx, nu, Np, Nc;
-    size_t admm_bytes, ric_bytes; int code_stride;
-    void (*fill)(const double* hs, const BmpcSysOff& o, void* pa, void* pp);
-    int view_fields; void (*fill_view)(struct bmpc_handle* h);
-    int view_ad, view_bd;              // field numbers of Ad and Bd in the per-instance parameter view (k_sys_refresh)
-    int (*configure)();
+    unsigned long long amask; unsigned bmask;   // (Ad, Bd) entries the kernels may find non-zero (all ones: any system)
+    size_t par_bytes;                  // host copy of the parameters (single-input: k_tpi_admm's block, then k_tpi_pol's)
+    int slots;                         // multi-input: gain slots per lane of the workspace
+    bool (*fill)(const double* hs, const BmpcSysOff& o, void* par);   // from system 0's block; false: declines (QDu not diagonal)
+    int view_fields, view_ad, view_bd; // per-instance parameter view: doubles per instance, field numbers of Ad and Bd (k_sys_refresh)
+    void (*fill_view)(struct bmpc_handle* h);
+    int (*configure)();                // single-input: shared-memory opt-in of its kernels (nullptr: none)
     void (*launch)(struct bmpc_handle* h, const int32_t* list, int count, const BmpcRoundPlan& p, int32_t* next_list);
 };
 
@@ -1130,21 +1119,18 @@ struct bmpc_handle {
     void (*tile_fn[3])(BmpcDims, BmpcSysOff, const double*, BmpcInst, const int32_t*, int, int, int, int, int, int) = {nullptr, nullptr, nullptr};   // tiles of 8, 4, 2
     struct { const int32_t* list; int count; int32_t *cur, *nxt; int total, chunk, round; bool need_prep; int tight; bool cold; } st = {};
     bool pending = false;              // a round is in flight and has not been retired by the host yet
-    int tpi_kind = 0;                  // 0 none, else 1 + index into g_tpi_table (compiled fast-path shapes)
-    void *tpi_admm_params = nullptr, *tpi_polish_params = nullptr;   // host copies of the parameter blocks
-    // the fast path's per-instance parameter blocks (n_sys = batch; TpiPolView or TpmPolView): field f of instance i at p[f * B + i].
-    // Recorded once at setup by whichever fast path owns it; bmpc_update_problem writes Ad / Bd into fields ad / bd (k_sys_refresh)
-    // and rebuilds the rest with fill
-    struct { double* p; int fields, ad, bd; void (*fill)(bmpc_handle* h); } view = {};
+    const BmpcFastEntry* fast = nullptr;   // the fast-path entry the handle runs on (select_fast); nullptr: the team kernels
+    void* fast_par = nullptr;          // host copy of its parameters
+    // the fast path's per-instance parameter blocks (n_sys = batch; TpiPolView or TpmPolView): field f of instance i at p[f * B + i],
+    // in the layout of entry e.  Recorded once at setup; bmpc_update_problem writes Ad / Bd into fields e->view_ad / view_bd
+    // (k_sys_refresh) and rebuilds the rest with e->fill_view
+    struct { double* p; const BmpcFastEntry* e; } view = {};
     bool codes_valid = false;         // the stored working sets come from a fast-path polish of the whole batch
-    int tpm_kind = 0;                  // 0 none, else 1 + index into g_tpm_table (compiled multi-input fast-path shapes)
-    void* tpm_params = nullptr;        // host copy of the parameter block
     double* tpm_W = nullptr; unsigned long long* tpm_rec = nullptr;   // gain rows of the resident warps, working-set records
     int tpm_W_slots = 0;               // gain slots per lane tpm_W was allocated for
-    // per-instance systems on the multi-input fast path (tpm_view_handle): the union of the instances' (Ad, Bd) patterns and whether
-    // some instance's QDu is not diagonal decide the entry (tpm_select_view).  tpm_word (device) / tpm_hword (pinned host): the
-    // pattern words of a device update [0] Ad, [1] Bd, and [2] the "QDu not diagonal" flag of k_tpm_fill_view
-    bool tpm_pi = false;
+    // per-instance systems on a multi-input view: the union of the instances' (Ad, Bd) patterns and whether some instance's QDu is not
+    // diagonal decide the entry (select_fast).  tpm_word (device) / tpm_hword (pinned host): the pattern words of a device update
+    // [0] Ad, [1] Bd, and [2] the "QDu not diagonal" flag of k_fill_view
     unsigned long long tpm_am = 0ull; unsigned tpm_bm = 0u; bool tpm_nondiag = false;
     unsigned long long *tpm_word = nullptr, *tpm_hword = nullptr;
     BmpcPolicy policy = {};            // round policy of the chosen kernel family (bmpc_rounds.cuh)
@@ -1170,10 +1156,14 @@ static std::string g_create_err;
         }                                                                                          \
     } while (0)
 
+// host copy of a single-input entry's parameters: the constant-bank blocks of k_tpi_admm and k_tpi_pol
+template <class S>
+struct TpiHostParams { TpiAdmmParams<S> admm; TpiPolParams<S> pol; };
+
 template <class S>
 static void launch_tpi_pol(bmpc_handle* h, const int32_t* list, int count, int mode, int capA, int capB, int reset, int32_t* next_list) {
     using L = TpiPolLayout<S>;
-    const TpiPolParams<S>& PP = *(const TpiPolParams<S>*)h->tpi_polish_params;
+    const TpiPolParams<S>& PP = ((const TpiHostParams<S>*)h->fast_par)->pol;
     TpiPolArgs A;
     A.list = list; A.count = count; A.mode = mode; A.capA = capA; A.capB = capB; A.reset = reset;
     A.next_list = next_list; A.counts = h->counts + BMPC_CNT * h->cpar; A.counts_next = h->counts + BMPC_CNT * (1 - h->cpar); A.queue = h->queue; A.qcap = h->cfg.batch; A.u0_out = h->I.u0; A.um1_solved = h->um1_solved;
@@ -1204,7 +1194,7 @@ template <class S>
 static void launch_tpi(bmpc_handle* h, const int32_t* list, int count, const BmpcRoundPlan& p, int32_t* next_list) {
     if (p.admm == BMPC_ADMM_TPI) {
         const int grid = (count + 31) / 32;
-        const TpiAdmmParams<S>& PA = *(const TpiAdmmParams<S>*)h->tpi_admm_params;
+        const TpiAdmmParams<S>& PA = ((const TpiHostParams<S>*)h->fast_par)->admm;
         const int cold = h->cold ? 1 : 0;
         const size_t sa = S::MT * TPI_STR * 8;
         if (h->xref_mode)   // one (Np+1) x nx reference per instance
@@ -1218,18 +1208,11 @@ static void launch_tpi(bmpc_handle* h, const int32_t* list, int count, const Bmp
 }
 
 template <class S>
-static void tpi_fill_entry(const double* hs, const BmpcSysOff& o, void* pa, void* pp) {
-    tpi_fill_admm<S>(hs, o, *(TpiAdmmParams<S>*)pa); tpi_fill_pol<S>(hs, o, *(TpiPolParams<S>*)pp);
+static bool tpi_fill_entry(const double* hs, const BmpcSysOff& o, void* par) {
+    TpiHostParams<S>& P = *(TpiHostParams<S>*)par;
+    tpi_fill_admm<S>(hs, o, P.admm); tpi_fill_pol<S>(hs, o, P.pol);
+    return true;
 }
-template <class S>
-static void tpi_fill_view_entry(bmpc_handle* h) {
-    const int B = h->cfg.batch;
-    k_tpi_fill_view<S><<<(B + 63) / 64, 64, 0, h->stream>>>(h->o, h->sys, (size_t)h->o.total, B, h->view.p);
-}
-template <class S>
-static constexpr int tpi_view_field_ad() { using PS = TpiPolParams<S>; return (int)(offsetof(PS, Ad) / sizeof(double)); }
-template <class S>
-static constexpr int tpi_view_field_bd() { using PS = TpiPolParams<S>; return (int)(offsetof(PS, Bd) / sizeof(double)); }
 template <class S>
 static int tpi_configure_entry() {
     if (cudaFuncSetAttribute(k_tpi_admm<S, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(S::MT * TPI_STR * 8)) != cudaSuccess) return 1;
@@ -1241,43 +1224,28 @@ static int tpi_configure_entry() {
     if (cudaFuncSetAttribute(k_tpi_pol<S, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm) != cudaSuccess) return 1;
     return 0;
 }
-#define BMPC_TPI_SHAPE(NX_, NU_, NP_, NC_)                                                                                   \
-    {NX_, NU_, NP_, NC_, sizeof(TpiAdmmParams<TpiShape<NX_, NU_, NP_, NC_>>), sizeof(TpiPolParams<TpiShape<NX_, NU_, NP_, NC_>>), \
-     TpiPolLayout<TpiShape<NX_, NU_, NP_, NC_>>::code_stride,                                                                \
-     tpi_fill_entry<TpiShape<NX_, NU_, NP_, NC_>>, TpiPolView<TpiShape<NX_, NU_, NP_, NC_>>::NF, tpi_fill_view_entry<TpiShape<NX_, NU_, NP_, NC_>>, \
-     tpi_view_field_ad<TpiShape<NX_, NU_, NP_, NC_>>(), tpi_view_field_bd<TpiShape<NX_, NU_, NP_, NC_>>(),                   \
-     tpi_configure_entry<TpiShape<NX_, NU_, NP_, NC_>>, launch_tpi<TpiShape<NX_, NU_, NP_, NC_>>},
-// BMPC_TPI_SHAPES_FILE: pympc_b200.build.jit_shape() compiles a copy of the library whose table holds the one shape a controller
-// asked for (any nx, Np with nu == 1) when the in-tree table does not have it
-#ifndef BMPC_TPI_SHAPES_FILE
-#define BMPC_TPI_SHAPES_FILE "tpi_shapes.inc"
-#endif
-static const TpiEntry g_tpi_table[] = {
-#include BMPC_TPI_SHAPES_FILE
-};
-#undef BMPC_TPI_SHAPE
-static const int g_tpi_count = (int)(sizeof(g_tpi_table) / sizeof(g_tpi_table[0]));
 
+// k_tpm_pol of a round.  Its first launch resets the instances itself when no ADMM ran before it in the round
 template <class S>
-static void launch_tpm(bmpc_handle* h, const int32_t* list, int count, int mode, int cap, int reset, int32_t* next_list, int exchange) {
+static void launch_tpm(bmpc_handle* h, const int32_t* list, int count, const BmpcRoundPlan& p, int32_t* next_list) {
     TpmArgs A;
-    A.list = list; A.count = count; A.mode = mode; A.cap = cap; A.reset = reset;
+    A.list = list; A.count = count; A.mode = p.ws; A.cap = p.cap; A.reset = p.admm == BMPC_ADMM_NONE ? p.reset : 0;
     A.counts = h->counts + BMPC_CNT * h->cpar; A.next_list = next_list; A.u0_out = h->I.u0; A.um1_solved = h->um1_solved;
     A.W = h->tpm_W; A.rec = h->tpm_rec; A.rec_stride = S::Np + 2;
     A.pview = h->view.p; A.pstride = h->cfg.batch;
-    const TpmParams<S>& P = *(const TpmParams<S>*)h->tpm_params;
+    const TpmParams<S>& P = *(const TpmParams<S>*)h->fast_par;
     const int grid = (count + 31) / 32;
     // exchange: the straggler rounds' instantiation (hard rows change by single exchanges, tpm_forward<S, true>); per-instance
-    // systems (h->tpm_pi): the instantiation that reads each instance's view
-    if (h->tpm_pi) {
-        if (exchange) {
+    // systems (a view): the instantiation that reads each instance's view
+    if (h->view.p) {
+        if (p.exchange) {
             if (h->xref_mode) k_tpm_pol<S, true, true, true><<<grid, 32, 0, h->stream>>>(P, h->I, A);
             else k_tpm_pol<S, false, true, true><<<grid, 32, 0, h->stream>>>(P, h->I, A);
         } else {
             if (h->xref_mode) k_tpm_pol<S, true, false, true><<<grid, 32, 0, h->stream>>>(P, h->I, A);
             else k_tpm_pol<S, false, false, true><<<grid, 32, 0, h->stream>>>(P, h->I, A);
         }
-    } else if (exchange) {
+    } else if (p.exchange) {
         if (h->xref_mode) k_tpm_pol<S, true, true, false><<<grid, 32, 0, h->stream>>>(P, h->I, A);
         else k_tpm_pol<S, false, true, false><<<grid, 32, 0, h->stream>>>(P, h->I, A);
     } else {
@@ -1287,40 +1255,58 @@ static void launch_tpm(bmpc_handle* h, const int32_t* list, int count, int mode,
     h->stats.launches++;
 }
 template <class S>
-static bool tpm_fill_entry(const double* hs, const BmpcSysOff& o, void* pp) { return tpm_fill<S>(hs, o, *(TpmParams<S>*)pp); }
-template <class S>
-static void tpm_fill_view_entry(bmpc_handle* h) {
+static bool tpm_fill_entry(const double* hs, const BmpcSysOff& o, void* par) { return tpm_fill<S>(hs, o, *(TpmParams<S>*)par); }
+
+// rebuilds the handle's view from every instance's block (PS: the parameter block of its entry); a multi-input view also gets the
+// "QDu not diagonal" word tpm_word[2] (allocated with such a view only)
+template <class PS>
+static void fill_view_entry(bmpc_handle* h) {
     const int B = h->cfg.batch;
-    cudaMemsetAsync(h->tpm_word + 2, 0, sizeof(unsigned long long), h->stream);
-    k_tpm_fill_view<S><<<(B + 63) / 64, 64, 0, h->stream>>>(h->o, h->sys, (size_t)h->o.total, B, h->view.p, h->tpm_word + 2);
+    unsigned long long* nondiag = h->tpm_word ? h->tpm_word + 2 : nullptr;
+    if (nondiag) cudaMemsetAsync(nondiag, 0, sizeof(unsigned long long), h->stream);
+    k_fill_view<PS><<<(B + 63) / 64, 64, 0, h->stream>>>(h->o, h->sys, (size_t)h->o.total, B, h->view.p, nondiag);
+}
+template <class PS>
+static constexpr int view_field_ad() { return (int)(offsetof(PS, Ad) / sizeof(double)); }
+template <class PS>
+static constexpr int view_field_bd() { return (int)(offsetof(PS, Bd) / sizeof(double)); }
+
+template <class S>
+static constexpr BmpcFastEntry tpi_entry() {
+    using PS = TpiPolParams<S>;
+    return {BMPC_FAM_TPI, S::nx, S::nu, S::Np, S::Nc, S::amask, S::bmask, sizeof(TpiHostParams<S>), 0, tpi_fill_entry<S>,
+            (int)(sizeof(PS) / sizeof(double)), view_field_ad<PS>(), view_field_bd<PS>(), fill_view_entry<PS>, tpi_configure_entry<S>, launch_tpi<S>};
 }
 template <class S>
-static constexpr int tpm_view_field_ad() { using PS = TpmParams<S>; return (int)(offsetof(PS, Ad) / sizeof(double)); }
-template <class S>
-static constexpr int tpm_view_field_bd() { using PS = TpmParams<S>; return (int)(offsetof(PS, Bd) / sizeof(double)); }
-#define BMPC_TPM_ENTRY(S_) {S_::nx, S_::nu, S_::Np, S_::Nc, S_::amask, S_::bmask, sizeof(TpmParams<S_>), TpmLayout<S_>::slots, tpm_fill_entry<S_>, \
-                            TpmPolView<S_>::NF, tpm_fill_view_entry<S_>, tpm_view_field_ad<S_>(), tpm_view_field_bd<S_>(), launch_tpm<S_>},
-#define BMPC_TPM_SHAPE(NX_, NU_, NP_, NC_) BMPC_TPM_ENTRY(BMPC_TPM_T4(TpiShape, NX_, NU_, NP_, NC_))
-#define BMPC_TPM_SPARSE_SHAPE(NX_, NU_, NP_, NC_, AM_, BM_) BMPC_TPM_ENTRY(BMPC_TPM_T6(TpmSparseShape, NX_, NU_, NP_, NC_, AM_, BM_))
-#define BMPC_TPM_T4(T_, a, b, c, d) T_<a, b, c, d>
-#define BMPC_TPM_T6(T_, a, b, c, d, e, f) T_<a, b, c, d, e, f>
-// (entries are tried in order: sparse patterns first, the dense instantiation of a shape last)
+static constexpr BmpcFastEntry tpm_entry() {
+    using PS = TpmParams<S>;
+    return {BMPC_FAM_TPM, S::nx, S::nu, S::Np, S::Nc, S::amask, S::bmask, sizeof(PS), TpmLayout<S>::slots, tpm_fill_entry<S>,
+            (int)(sizeof(PS) / sizeof(double)), view_field_ad<PS>(), view_field_bd<PS>(), fill_view_entry<PS>, nullptr, launch_tpm<S>};
+}
+// BMPC_TPI_SHAPES_FILE / BMPC_TPM_SHAPES_FILE: pympc_b200.build.jit_shape() / jit_multi_input_shape() compile a copy of the library
+// whose table holds the one shape a controller asked for when the in-tree table does not have it.  Entries are tried in order:
+// single-input shapes first; of a multi-input shape the sparse patterns first, its dense instantiation last
+#define BMPC_TPI_SHAPE(NX_, NU_, NP_, NC_) tpi_entry<TpiShape<NX_, NU_, NP_, NC_>>(),
+#define BMPC_TPM_SHAPE(NX_, NU_, NP_, NC_) tpm_entry<TpiShape<NX_, NU_, NP_, NC_>>(),
+#define BMPC_TPM_SPARSE_SHAPE(NX_, NU_, NP_, NC_, AM_, BM_) tpm_entry<TpmSparseShape<NX_, NU_, NP_, NC_, AM_, BM_>>(),
+#ifndef BMPC_TPI_SHAPES_FILE
+#define BMPC_TPI_SHAPES_FILE "tpi_shapes.inc"
+#endif
 #ifndef BMPC_TPM_SHAPES_FILE
 #define BMPC_TPM_SHAPES_FILE "tpm_shapes.inc"
 #endif
-static const TpmEntry g_tpm_table[] = {
+static const BmpcFastEntry g_fast[] = {
+#include BMPC_TPI_SHAPES_FILE
 #include BMPC_TPM_SHAPES_FILE
 };
+#undef BMPC_TPI_SHAPE
 #undef BMPC_TPM_SHAPE
 #undef BMPC_TPM_SPARSE_SHAPE
-static const int g_tpm_count = (int)(sizeof(g_tpm_table) / sizeof(g_tpm_table[0]));
 
-// index of the first entry at or after `from` of a compiled table (g_tpi_table, g_tpm_table) with d's (nx, nu, Np, Nc); -1: none
-template <class E>
-static int find_shape(const E* table, int count, const BmpcDims& d, int from = 0) {
-    for (int k = from; k < count; k++)
-        if (table[k].nx == d.nx && table[k].nu == d.nu && table[k].Np == d.Np && table[k].Nc == d.Nc) return k;
-    return -1;
+static bool same_shape(const BmpcFastEntry& e, const BmpcDims& d) { return e.nx == d.nx && e.nu == d.nu && e.Np == d.Np && e.Nc == d.Nc; }
+static bool has_entry(int family, const BmpcDims& d) {
+    for (const BmpcFastEntry& e : g_fast) if (e.family == family && same_shape(e, d)) return true;
+    return false;
 }
 
 extern "C" {
@@ -1336,11 +1322,11 @@ void bmpc_default_config(bmpc_config* c) {
 }
 
 int bmpc_has_fast_path(int nx, int nu, int Np, int Nc) {
-    return find_shape(g_tpi_table, g_tpi_count, bmpc_make_dims(nx, nu, Np, Nc <= 0 ? Np : Nc)) >= 0;
+    return has_entry(BMPC_FAM_TPI, bmpc_make_dims(nx, nu, Np, Nc <= 0 ? Np : Nc));
 }
 
 int bmpc_has_multi_input_fast_path(int nx, int nu, int Np, int Nc) {
-    return find_shape(g_tpm_table, g_tpm_count, bmpc_make_dims(nx, nu, Np, Nc <= 0 ? Np : Nc)) >= 0;
+    return has_entry(BMPC_FAM_TPM, bmpc_make_dims(nx, nu, Np, Nc <= 0 ? Np : Nc));
 }
 
 int bmpc_device_count(void) {
@@ -1440,7 +1426,7 @@ int bmpc_create(const bmpc_config* cfg, bmpc_handle** out) {
     ok &= dalloc((void**)&h->listB, sizeof(int32_t) * B);
     ok &= dalloc((void**)&h->counts, sizeof(int32_t) * 2 * BMPC_CNT);
     ok &= dalloc((void**)&h->queue, sizeof(int32_t) * B);
-    h->code_stride = tpi_code_stride(d.nx, d.Np);          // the record of this shape's fast-path entry (bmpc_setup checks it)
+    h->code_stride = tpi_code_stride(d.nx, d.Np);          // the record of this shape's single-input entry (TpiPolLayout asserts it)
     ok &= dalloc((void**)&h->codes, (size_t)B * h->code_stride);
     ok &= dalloc((void**)&h->ovf, sizeof(int32_t) * (size_t)B);
     ok &= dalloc((void**)&h->vprev, sizeof(double) * (size_t)B * d.mc);
@@ -1475,7 +1461,7 @@ void bmpc_destroy(bmpc_handle* h) {
                     h->I.status, h->I.iters, h->I.psteps, h->I.lvl, h->listA, h->listB, h->counts, h->queue, h->codes, h->ovf, h->vprev, h->lprev, h->seq_x, h->seq_e, h->seq_obj};
     for (void* p : ptrs) if (p) cudaFree(p);
     if (h->h_count) cudaFreeHost(h->h_count);
-    free(h->tpi_admm_params); free(h->tpi_polish_params); free(h->tpm_params);
+    free(h->fast_par);
     if (h->view.p) cudaFree(h->view.p);
     if (h->tpm_word) cudaFree(h->tpm_word);
     if (h->tpm_hword) cudaFreeHost(h->tpm_hword);
@@ -1611,11 +1597,6 @@ static int check_condensed(bmpc_handle* h, const char* who) {
     return BMPC_OK;
 }
 
-// multi-input fast path: compiled shape, soft state rows, polish on (shared systems: bmpc_setup / derive_from_block; per-instance
-// systems: tpm_select_view)
-static bool tpm_eligible(const bmpc_handle* h) {
-    return h->cfg.fast_path && !h->tpi_kind && h->cfg.soft_on && h->cfg.polish;
-}
 // the (Ad, Bd) sparsity pattern of n systems (system i's Ad at Ad[i * stride], Bd at Bd[i * stride]), as the union over them: bit
 // q nx + b of *am: Ad[q][b] non-zero in some system, bit a nu + j of *bm: Bd[a][j].  Shapes beyond the masks: all bits
 static void tpm_pattern(const BmpcDims& d, const double* Ad, const double* Bd, int n, size_t stride, unsigned long long* am, unsigned* bm) {
@@ -1626,69 +1607,62 @@ static void tpm_pattern(const BmpcDims& d, const double* Ad, const double* Bd, i
         if (Bd) for (int i = 0; i < d.nx * d.nu; i++) if (Bd[s * stride + i] != 0.0) *bm |= 1u << i;
     }
 }
-// the first compiled entry of the shape whose pattern masks contain the pattern (am, bm); 0: none
-static int tpm_match(const BmpcDims& d, unsigned long long am, unsigned bm) {
-    for (int k = find_shape(g_tpm_table, g_tpm_count, d); k >= 0; k = find_shape(g_tpm_table, g_tpm_count, d, k + 1))
-        if ((am & ~g_tpm_table[k].amask) == 0ull && (bm & ~g_tpm_table[k].bmask) == 0u) return k + 1;
-    return 0;
-}
-static bool tpm_sparse(int kind) { return kind && (~g_tpm_table[kind - 1].amask || ~g_tpm_table[kind - 1].bmask); }
-// gain rows and working-set records of multi-input entry `kind`.  fresh: the stored records start empty (the next warm solve reads
-// its working sets off v*)
-static int tpm_alloc(bmpc_handle* h, int kind, bool fresh) {
-    const TpmEntry& te = g_tpm_table[kind - 1];
+// gain rows and working-set records of multi-input entry e.  fresh: the stored records start empty (the next warm solve reads its
+// working sets off v*)
+static int tpm_alloc(bmpc_handle* h, const BmpcFastEntry& e, bool fresh) {
     const size_t B = h->cfg.batch, nwarp = (B + 31) / 32;
-    if (h->tpm_W && h->tpm_W_slots < te.slots) { cudaFree(h->tpm_W); h->tpm_W = nullptr; }
-    if (!h->tpm_W) { BMPC_CUDA(cudaMalloc((void**)&h->tpm_W, sizeof(double) * nwarp * 32 * (size_t)te.slots)); h->tpm_W_slots = te.slots; }
+    if (h->tpm_W && h->tpm_W_slots < e.slots) { cudaFree(h->tpm_W); h->tpm_W = nullptr; }
+    if (!h->tpm_W) { BMPC_CUDA(cudaMalloc((void**)&h->tpm_W, sizeof(double) * nwarp * 32 * (size_t)e.slots)); h->tpm_W_slots = e.slots; }
     if (!h->tpm_rec) { BMPC_CUDA(cudaMalloc((void**)&h->tpm_rec, sizeof(unsigned long long) * B * (size_t)(h->d.Np + 2))); fresh = true; }
     if (fresh) BMPC_CUDA(cudaMemsetAsync(h->tpm_rec, 0, sizeof(unsigned long long) * B * (size_t)(h->d.Np + 2), h->stream));
     return BMPC_OK;
 }
 
 static int policy_family(const bmpc_handle* h) {
-    return h->tpi_kind ? (h->view.p ? BMPC_FAM_TPI_VIEW : BMPC_FAM_TPI) : h->tpm_kind ? BMPC_FAM_TPM : BMPC_FAM_TEAM;
+    if (!h->fast) return BMPC_FAM_TEAM;
+    return h->fast->family == BMPC_FAM_TPI && h->view.p ? BMPC_FAM_TPI_VIEW : h->fast->family;
 }
 
-// what the host derives from system 0's condensed block (bmpc_setup; bmpc_update_problem on a shared system): the single-input fast
-// path's constant-bank parameters, the multi-input entry and the kernel family.  Reads the block back only when a fast path is in play
-// (the single-input one, or multi-input entries of this shape: their pattern match reads Ad, Bd).  fresh: empty multi-input records.
-// The multi-input entry stays off when its fill declines (QDu not diagonal: team kernels).  (Per-instance systems: tpm_select_view)
-static int derive_from_block(bmpc_handle* h, bool fresh) {
-    const int old = h->tpm_kind;
-    const bool tpm = tpm_eligible(h) && h->cfg.n_sys <= 1 && find_shape(g_tpm_table, g_tpm_count, h->d) >= 0;
-    h->tpm_kind = 0;
-    if (h->tpi_kind || tpm) {
-        std::vector<double> hs(h->o.total);
-        BMPC_CUDA(cudaMemcpyAsync(hs.data(), h->sys, sizeof(double) * h->o.total, cudaMemcpyDeviceToHost, h->stream));
-        BMPC_CUDA(cudaStreamSynchronize(h->stream));
-        if (h->tpi_kind) g_tpi_table[h->tpi_kind - 1].fill(hs.data(), h->o, h->tpi_admm_params, h->tpi_polish_params);
-        unsigned long long am; unsigned bm;
-        tpm_pattern(h->d, hs.data() + h->o.Ad, hs.data() + h->o.Bd, 1, 0, &am, &bm);
-        const int tk = tpm ? tpm_match(h->d, am, bm) : 0;
-        if (tk) {
-            free(h->tpm_params); h->tpm_params = malloc(g_tpm_table[tk - 1].par_bytes);
-            if (g_tpm_table[tk - 1].fill(hs.data(), h->o, h->tpm_params)) {
-                h->tpm_kind = tk;
-                int rc = tpm_alloc(h, tk, fresh || tk != old); if (rc) return rc;
-            }
+// the options let entry e take the handle's system, whatever its pattern: the handle's shape, fast_path, soft state rows (the Riccati
+// polishes treat state rows as the soft penalty they are by default), and one-warp teams (single-input) or polish on (multi-input)
+static bool fast_allowed(const bmpc_handle* h, const BmpcFastEntry& e) {
+    const bmpc_config& c = h->cfg;
+    return same_shape(e, h->d) && c.fast_path && c.soft_on && (e.family == BMPC_FAM_TPI ? h->launch.team == 32 : c.polish != 0);
+}
+
+// The fast-path entry of the handle (h->fast, nullptr: the team kernels), its parameters and the kernel family: the first entry of
+// the table the options allow (fast_allowed) and that takes the system.  A single-input entry takes any system; a multi-input entry
+// one whose (Ad, Bd) pattern its masks contain and whose QDu is diagonal.  Shared system: pattern and diagonality of system 0's block,
+// read back only when the options allow some entry (the fill reports QDu).  Per-instance systems: the union the handle keeps over the
+// instances (tpm_am, tpm_bm, tpm_nondiag); a multi-input entry reads only the view, and the block comes back only for a single-input
+// entry's constant-bank fill.  The multi-input records restart empty when the entry changes or the caller asks for fresh ones.
+static int select_fast(bmpc_handle* h, bool fresh) {
+    const bool shared = h->cfg.n_sys <= 1;
+    std::vector<double> hs;
+    for (const BmpcFastEntry& e : g_fast)
+        if (fast_allowed(h, e) && (shared || e.family == BMPC_FAM_TPI)) {
+            hs.resize(h->o.total);
+            BMPC_CUDA(cudaMemcpyAsync(hs.data(), h->sys, sizeof(double) * h->o.total, cudaMemcpyDeviceToHost, h->stream));
+            BMPC_CUDA(cudaStreamSynchronize(h->stream));
+            break;
         }
+    unsigned long long am = h->tpm_am; unsigned bm = h->tpm_bm;
+    if (shared && !hs.empty()) tpm_pattern(h->d, hs.data() + h->o.Ad, hs.data() + h->o.Bd, 1, 0, &am, &bm);
+    if (!h->fast_par) {                                   // one host copy for whichever entry the handle takes: the largest
+        size_t bytes = 0;
+        for (const BmpcFastEntry& e : g_fast) bytes = e.par_bytes > bytes ? e.par_bytes : bytes;
+        h->fast_par = calloc(1, bytes);
     }
-    h->policy.family = policy_family(h);
-    return BMPC_OK;
-}
-
-// per-instance systems on the multi-input fast path: the entry whose masks contain the union of the instances' patterns (tpm_am,
-// tpm_bm), none while some instance's QDu is not diagonal (team kernels).  The view itself is kept current by the caller (setup and
-// every update fill it, whichever family runs), so a change of entry needs only the workspace; it starts with empty records, as after
-// setup (fresh).
-static int tpm_select_view(bmpc_handle* h, bool fresh) {
-    const int old = h->tpm_kind;
-    const int kind = h->tpm_nondiag ? 0 : tpm_match(h->d, h->tpm_am, h->tpm_bm);
-    h->tpm_kind = kind;
-    if (kind) {
-        if (!h->tpm_params) h->tpm_params = calloc(1, g_tpm_table[kind - 1].par_bytes);     // (k_tpm_pol<..., PERINST> reads the view)
-        int rc = tpm_alloc(h, kind, fresh || kind != old); if (rc) return rc;
+    const BmpcFastEntry* old = h->fast;
+    h->fast = nullptr;
+    for (const BmpcFastEntry& e : g_fast) {
+        if (!fast_allowed(h, e)) continue;
+        if (e.family == BMPC_FAM_TPM && (h->tpm_nondiag || (am & ~e.amask) || (bm & ~e.bmask))) continue;
+        if (!hs.empty() && !e.fill(hs.data(), h->o, h->fast_par)) continue;
+        h->fast = &e;
+        break;
     }
+    if (h->fast && h->fast->family == BMPC_FAM_TPM) { int rc = tpm_alloc(h, *h->fast, fresh || h->fast != old); if (rc) return rc; }
     h->policy.family = policy_family(h);
     return BMPC_OK;
 }
@@ -1722,49 +1696,30 @@ int bmpc_setup(bmpc_handle* h, const double* Ad, const double* Bd, const double*
     BMPC_CUDA(cudaGetLastError());
     // everything derived from the new arrays comes before the check: a handle refused after a failed setup still describes what its
     // blocks hold, so a later update decides and refreshes from the same state as after a failed update
-    // thread-per-instance fast path for the compiled small shapes (pendulum, point mass)
-    // (the Riccati polish treats state rows as the soft penalty they are by default; hard state rows -> team kernels)
-    h->tpi_kind = h->cfg.fast_path && h->launch.team == 32 && h->cfg.soft_on ? find_shape(g_tpi_table, g_tpi_count, d) + 1 : 0;
-    if (h->tpi_kind) {
-        const TpiEntry& te = g_tpi_table[h->tpi_kind - 1];
-        if (te.code_stride > h->code_stride) { h->err = "fast path: working-set record larger than allocated"; return BMPC_ERR_STATE; }
-        free(h->tpi_admm_params); free(h->tpi_polish_params);
-        h->tpi_admm_params = malloc(te.admm_bytes); h->tpi_polish_params = malloc(te.ric_bytes);
-        if (te.configure()) { h->err = "fast path: shared-memory configuration failed"; return BMPC_ERR_CUDA; }
-        if (h->view.p) { cudaFree(h->view.p); h->view = {}; }
-        if (ns > 1) {
-            // one parameter block per instance, built on the device from each instance's condensed system block
-            BMPC_CUDA(cudaMalloc((void**)&h->view.p, sizeof(double) * (size_t)te.view_fields * h->cfg.batch));
-            h->view.fields = te.view_fields; h->view.ad = te.view_ad; h->view.bd = te.view_bd; h->view.fill = te.fill_view;
-            te.fill_view(h);
-            BMPC_CUDA(cudaGetLastError());
-        }
-    }
-    // the fast paths' parameters and the kernel family; multi-input fast path: compiled shape, soft state rows, diagonal QDu
-    // (sparsity pattern of (Ad, Bd): an entry fits when its compile-time masks contain it)
-    int rc = derive_from_block(h, true);
-    if (rc) return rc;
-    // per-instance systems on the multi-input fast path: the view is kept whichever family runs (a later update may bring the
-    // handle onto an entry); the entry matches the union of the instances' patterns, and every QDu must be diagonal
-    const int tpm_shape = find_shape(g_tpm_table, g_tpm_count, d);
-    h->tpm_pi = ns > 1 && tpm_eligible(h) && tpm_shape >= 0;
-    if (h->tpm_pi) {
-        const TpmEntry& te = g_tpm_table[tpm_shape];
+    // per-instance systems: one parameter block per instance, built on the device from each instance's block, in the layout of the
+    // first entry the options allow (a single-input shape: its entry; a multi-input shape: its first entry).  It is kept current
+    // whichever family runs (a later update may bring the handle onto a multi-input entry)
+    const BmpcFastEntry* ve = nullptr;
+    if (ns > 1) for (const BmpcFastEntry& e : g_fast) if (fast_allowed(h, e)) { ve = &e; break; }
+    if (ve && ve->family == BMPC_FAM_TPM) {
         if (!h->tpm_word) BMPC_CUDA(cudaMalloc((void**)&h->tpm_word, 3 * sizeof(unsigned long long)));
         if (!h->tpm_hword) BMPC_CUDA(cudaMallocHost((void**)&h->tpm_hword, 3 * sizeof(unsigned long long)));
-        if (!h->view.p) BMPC_CUDA(cudaMalloc((void**)&h->view.p, sizeof(double) * (size_t)te.view_fields * h->cfg.batch));
-        h->view.fields = te.view_fields; h->view.ad = te.view_ad; h->view.bd = te.view_bd; h->view.fill = te.fill_view;
-        te.fill_view(h);
-        BMPC_CUDA(cudaGetLastError());
         tpm_pattern(d, in.data() + P[0].off, in.data() + P[1].off, ns, o.pw, &h->tpm_am, &h->tpm_bm);
         h->tpm_nondiag = false;
         for (int si = 0; si < ns; si++) {
             const double* q = in.data() + (size_t)si * o.pw + P[5].off;
             for (int i = 0; i < d.nu * d.nu; i++) if (i / d.nu != i % d.nu && q[i] != 0.0) h->tpm_nondiag = true;
         }
-        rc = tpm_select_view(h, true);
-        if (rc) return rc;
     }
+    if (ve) {
+        if (!h->view.p) BMPC_CUDA(cudaMalloc((void**)&h->view.p, sizeof(double) * (size_t)ve->view_fields * h->cfg.batch));
+        h->view.e = ve;
+        ve->fill_view(h);
+        BMPC_CUDA(cudaGetLastError());
+    }
+    int rc = select_fast(h, true);
+    if (rc) return rc;
+    if (h->fast && h->fast->configure && h->fast->configure()) { h->err = "fast path: shared-memory configuration failed"; return BMPC_ERR_CUDA; }
     const bmpc_config& c = h->cfg;
     h->policy = bmpc_make_policy(h->policy.family, c.polish, c.first_iters, c.cold_iters, c.max_iter, c.pdas_steps, c.shift_warm);
     // time-varying problem data on per-instance systems: when the weights keep H positive definite for ANY (Ad, Bd),
@@ -1836,7 +1791,7 @@ int bmpc_update_problem(bmpc_handle* h, const double* Ad, const double* Bd, cons
         BMPC_CUDA(cudaGetLastError());
         int rc = check_condensed(h, "bmpc_update_problem");
         if (rc) return rc;
-        rc = derive_from_block(h, false);
+        rc = select_fast(h, false);
         if (rc) return rc;
         h->sys_bad = false;
         return BMPC_OK;
@@ -1845,9 +1800,10 @@ int bmpc_update_problem(bmpc_handle* h, const double* Ad, const double* Bd, cons
     // to the launches that read a condensed block (condense_stale) — unless H may lose definiteness, then all of it now + the check
     const int B = h->cfg.batch;
     const bool hv = h->view.p != nullptr;                // the handle's parameter view (either fast path)
+    const bool tpm_view = hv && h->view.e->family == BMPC_FAM_TPM;
     if (!on_device && !h->sys_stage) BMPC_CUDA(cudaMalloc((void**)&h->sys_stage, sizeof(double) * (size_t)B * o.pw));
     BmpcRefreshTab T = {}; size_t per = 0;
-    bool view_fill = false;                              // an array the view holds only through derived fields (view.fill)
+    bool view_fill = false;                              // an array the view holds only through derived fields (fill_view)
     for (int f = 0; f < 13; f++) {
         if (!src[f]) continue;
         const double* s = src[f];
@@ -1855,7 +1811,7 @@ int bmpc_update_problem(bmpc_handle* h, const double* Ad, const double* Bd, cons
             BMPC_CUDA(cudaMemcpyAsync(h->sys_stage + (size_t)B * P[f].off, s, sizeof(double) * B * P[f].cnt, cudaMemcpyHostToDevice, h->stream));
             s = h->sys_stage + (size_t)B * P[f].off;
         }
-        const int view = !hv ? -1 : f == 0 ? h->view.ad : f == 1 ? h->view.bd : -1;
+        const int view = !hv ? -1 : f == 0 ? h->view.e->view_ad : f == 1 ? h->view.e->view_bd : -1;
         view_fill = view_fill || (hv && f >= 2);
         T.seg[T.n++] = BmpcRefreshSeg{s, P[f].off, P[f].cnt, view};
         per += (size_t)P[f].cnt;
@@ -1863,19 +1819,19 @@ int bmpc_update_problem(bmpc_handle* h, const double* Ad, const double* Bd, cons
     const size_t n = (size_t)B * per;
     k_sys_refresh<<<(unsigned)((n + 255) / 256), 256, 0, h->stream>>>(h->sys, h->I.sys_stride, B, T, h->view.p);
     BMPC_CUDA(cudaGetLastError());
-    if (view_fill) { h->view.fill(h); BMPC_CUDA(cudaGetLastError()); }
+    if (view_fill) { h->view.e->fill_view(h); BMPC_CUDA(cudaGetLastError()); }
     h->sys_gen_cur++; h->sys_stale = true;
     // multi-input fast path on per-instance systems: the union pattern of the new (Ad, Bd) and "QDu not diagonal" decide the entry
     // below.  Host arrays: decided here.  Device (Ad, Bd) on a sparse entry: k_tpm_pattern + one synchronising read of the pattern
     // words; on the dense entry or the team kernels the pattern is taken as dense (nothing is read back).  Device QDu: the flag
-    // k_tpm_fill_view raised, read in the synchronisation of the definiteness check below
-    const bool qdu_dev = h->tpm_pi && QDu && on_device;
-    if (h->tpm_pi && model) {
+    // k_fill_view raised, read in the synchronisation of the definiteness check below
+    const bool qdu_dev = tpm_view && QDu && on_device;
+    if (tpm_view && model) {
         if (!on_device) {
             unsigned long long am; unsigned bm;
             if (Ad) { tpm_pattern(d, Ad, nullptr, B, (size_t)P[0].cnt, &am, &bm); h->tpm_am = am; }
             if (Bd) { tpm_pattern(d, nullptr, Bd, B, (size_t)P[1].cnt, &am, &bm); h->tpm_bm = bm; }
-        } else if (tpm_sparse(h->tpm_kind)) {
+        } else if (h->fast && (~h->fast->amask || ~h->fast->bmask)) {        // a sparse entry
             BMPC_CUDA(cudaMemsetAsync(h->tpm_word, 0, 2 * sizeof(unsigned long long), h->stream));
             if (Ad) k_tpm_pattern<<<(B + 127) / 128, 128, 0, h->stream>>>(Ad, P[0].cnt, B, h->tpm_word);
             if (Bd) k_tpm_pattern<<<(B + 127) / 128, 128, 0, h->stream>>>(Bd, P[1].cnt, B, h->tpm_word + 1);
@@ -1889,7 +1845,7 @@ int bmpc_update_problem(bmpc_handle* h, const double* Ad, const double* Bd, cons
             if (Bd) h->tpm_bm = ~0u;
         }
     }
-    if (h->tpm_pi && QDu && !on_device) {
+    if (tpm_view && QDu && !on_device) {
         h->tpm_nondiag = false;
         for (int si = 0; si < B; si++)
             for (int i = 0; i < d.nu * d.nu; i++) if (i / d.nu != i % d.nu && QDu[(size_t)si * d.nu * d.nu + i] != 0.0) h->tpm_nondiag = true;
@@ -1913,9 +1869,9 @@ int bmpc_update_problem(bmpc_handle* h, const double* Ad, const double* Bd, cons
         BMPC_CUDA(cudaGetLastError());
         int rc = check_condensed(h, "bmpc_update_problem");
         if (qdu_dev) h->tpm_nondiag = h->tpm_hword[2] != 0ull;        // (check_condensed synchronised the stream)
-        if (rc) { if (h->tpm_pi) tpm_select_view(h, false); return rc; }   // refused; the entry still follows the arrays the blocks hold
+        if (rc) { if (tpm_view) select_fast(h, false); return rc; }   // refused; the entry still follows the arrays the blocks hold
     }
-    if (h->tpm_pi) { int rc = tpm_select_view(h, false); if (rc) return rc; }
+    if (tpm_view) { int rc = select_fast(h, false); if (rc) return rc; }
     // (bounds and uref alone leave definiteness as it was: a handle refused after a failed update stays refused)
     if (check || h->sys_lazy) h->sys_bad = false;
     return BMPC_OK;
@@ -1991,13 +1947,7 @@ static int enqueue_round(bmpc_handle* h, const BmpcRoundPlan& p) {
     if (p.admm == BMPC_ADMM_NONE && p.polish == BMPC_POL_TPI) { h->epoch = (h->epoch % 1000000000) + 1; h->spin_epoch = h->epoch; ((volatile int32_t*)h->h_count)[BMPC_CNT_EPOCH] = 0; }
     // (a warm fast-path round times itself with the global timer and reports through mapped memory: no event records in the stream)
     if (!h->spin_epoch) BMPC_CUDA(cudaEventRecord(h->ev[0], h->stream));
-    if (tpi_first) {
-        g_tpi_table[h->tpi_kind - 1].launch(h, st.list, st.count, p, st.nxt);
-        h->codes_valid = true;
-    } else if (!team) {
-        BMPC_CUDA(cudaEventRecord(h->ev[1], h->stream));
-        g_tpm_table[h->tpm_kind - 1].launch(h, st.list, st.count, p.ws, p.cap, p.reset, st.nxt, p.exchange);
-    } else {
+    if (team) {
         const BmpcRoundLaunch R = bmpc_round_launch(h->launch, h->d, st.count, st.list != nullptr, h->sm_count);
         if (p.infeas) { k_snapshot<<<st.count, 128, 0, h->stream>>>(h->d, h->I, st.list, st.count, h->vprev, h->lprev); h->stats.launches++; }
         launch_admm(h, R, st.list, st.count, p.chunk, st.need_prep ? 1 : 0);
@@ -2007,11 +1957,13 @@ static int enqueue_round(bmpc_handle* h, const BmpcRoundPlan& p) {
             h->stats.launches++;
         }
         BMPC_CUDA(cudaEventRecord(h->ev[1], h->stream));
-        if (p.polish == BMPC_POL_TPI) g_tpi_table[h->tpi_kind - 1].launch(h, st.list, st.count, p, st.nxt);
-        else if (p.polish == BMPC_POL_TPM) g_tpm_table[h->tpm_kind - 1].launch(h, st.list, st.count, p.ws, p.cap, 0, st.nxt, p.exchange);
-        else if (p.polish == BMPC_POL_SCHUR) launch_polish(h, R, st.list, st.count, p.cap, st.nxt, cnt);
-        else { k_check_converged<<<(st.count + 255) / 256, 256, 0, h->stream>>>(h->I, st.list, st.count, h->cfg.eps_abs, h->cfg.eps_rel, st.nxt, cnt); h->stats.launches++; }
+        if (p.polish == BMPC_POL_SCHUR) launch_polish(h, R, st.list, st.count, p.cap, st.nxt, cnt);
+        else if (p.polish == BMPC_POL_CHECK) { k_check_converged<<<(st.count + 255) / 256, 256, 0, h->stream>>>(h->I, st.list, st.count, h->cfg.eps_abs, h->cfg.eps_rel, st.nxt, cnt); h->stats.launches++; }
+    } else if (!tpi_first) {
+        BMPC_CUDA(cudaEventRecord(h->ev[1], h->stream));      // (k_tpi_admm, when a first round has it, records ev[1] behind itself)
     }
+    if (p.polish == BMPC_POL_TPI || p.polish == BMPC_POL_TPM) h->fast->launch(h, st.list, st.count, p, st.nxt);
+    if (tpi_first) h->codes_valid = true;
     h->I.um1 = h->um1_cur;
     if (!h->spin_epoch) BMPC_CUDA(cudaEventRecord(h->ev[2], h->stream));
     if (!h->spin_epoch) BMPC_CUDA(cudaMemcpyAsync(h->h_count, cnt, sizeof(int32_t) * BMPC_CNT, cudaMemcpyDeviceToHost, h->stream));

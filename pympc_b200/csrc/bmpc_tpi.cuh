@@ -685,7 +685,7 @@ BMPC_HD unsigned tpi2_shifted_code(const typename TpiCode<S>::type* stored, int 
 // The polish parameters of one system.  Reads only the system's inputs (Ad .. uref) and scal[RHO], scal[RHOE], never the condensed
 // arrays: the rows' bounds are the raw bounds (lo0 / hi0 copy them) and a row's rho follows the condense's rule (bmpc_row_rho).
 // So the fill stays valid on a block whose condensed part predates its inputs (per-instance systems after bmpc_update_problem,
-// k_tpi_fill_view), and gives bit for bit the block a fill from a freshly condensed system gives.
+// k_fill_view), and gives bit for bit the block a fill from a freshly condensed system gives.
 template <class S>
 BMPC_HOSTDEV void tpi_fill_pol(const double* sys, const BmpcSysOff& o, TpiPolParams<S>& P) {
     constexpr int nx = S::nx;

@@ -576,7 +576,7 @@ BMPC_HD int tpm_vstar_row(int k, int p) {
 // The parameters of one system; returns "QDu diagonal" (the sweeps need it).  Reads only the system's inputs (Ad .. uref) and
 // scal[RHO], scal[RHOE], never the condensed arrays: the rows' bounds are the raw bounds (lo0 / hi0 copy them, periodic in nu) and a
 // row's rho follows the condense's rule (bmpc_row_rho).  So the fill stays valid on a block whose condensed part predates its inputs
-// (per-instance systems after bmpc_update_problem, k_tpm_fill_view) and gives bit for bit what a fill of the freshly condensed block gives.
+// (per-instance systems after bmpc_update_problem, k_fill_view) and gives bit for bit what a fill of the freshly condensed block gives.
 template <class S>
 BMPC_HOSTDEV bool tpm_fill(const double* sys, const BmpcSysOff& o, TpmParams<S>& P) {
     constexpr int nx = S::nx, nu = S::nu;

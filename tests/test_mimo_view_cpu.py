@@ -60,7 +60,7 @@ def _rand_cfg(rng, shape, nondiag=False):
 
 @pytest.mark.parametrize("entry", sorted(ENTRIES))
 def test_tpm_fill_on_a_stale_block_equals_a_fresh_condense_bit_for_bit(entry, view_lib):
-    """k_tpm_fill_view after an update fills from the raw inputs of a block whose condensed part predates them: over random bounds
+    """k_fill_view after an update fills from the raw inputs of a block whose condensed part predates them: over random bounds
     (with +-inf rows, so that rows change between free and bounded), weights and uref it equals, bit for bit, the fill of the
     same block condensed afresh with the rho the setup chose.  "QDu diagonal" is reported the same way on both"""
     shape = ENTRIES[entry]
