@@ -208,6 +208,37 @@ int bmpc_est_set_stream(bmpc_estimator* e, void* cuda_stream);
  * a predict/update that takes a device pointer first retires the controller's deferred solve.  h = NULL detaches. */
 int bmpc_est_attach(bmpc_estimator* e, bmpc_handle* h);
 
+/* ---- batched Kalman filter: an estimator whose gain is computed every step (csrc/bmpc_kf.cuh), for models that change between
+ * steps.  Model of kalman_design_simple (kalman.py:73-106): x+ = A x + B u + w, E[ww'] = Qn; y = C x + v, E[vv'] = Rn.
+ *   predict(u):       x <- A x + B u;  P <- A P A' + Qn;  y <- C x
+ *   update(y_meas):   S = C P C' + Rn;  K = P C' S^-1 (Cholesky of S);  x <- x + K (y_meas - y);
+ *                     P <- (I - K C) P (I - K C)' + K Rn K', symmetrised
+ * x is the a-priori estimate x[k|k-1], where the reference's estimator sits after construction or predict; y is refreshed by
+ * predict only.  bmpc_est_predict / update / get / state_ptr / set_stream / attach / destroy apply unchanged.  1 <= nx, ny <= 32,
+ * nu >= 1; n_sys = 1 (shared model, held in shared memory) or batch (one model per instance).  A [n_sys,nx,nx], B [n_sys,nx,nu],
+ * C [n_sys,ny,nx], Qn [n_sys,nx,nx], Rn [n_sys,ny,ny], x0 [batch,nx], P0 [batch,nx,nx]: host pointers, row-major, batch-major.
+ * Qn, Rn and P0 are symmetric: their upper triangles (Rn: lower) are read.  The per-instance status of the last update is
+ * BMPC_KF_OK, or BMPC_KF_S_NOT_PD when S is not positive definite (a non-positive or non-finite Cholesky pivot): that instance's x
+ * and P are left as they were; the others are unaffected.  Before the first update the status is BMPC_KF_OK. */
+enum {
+    BMPC_KF_OK = 1,
+    BMPC_KF_S_NOT_PD = -2       /* innovation covariance S = C P C' + Rn not positive definite */
+};
+int bmpc_est_create_kf(int32_t nx, int32_t nu, int32_t ny, int32_t batch, int32_t n_sys, int32_t device, const double* A,
+                       const double* B, const double* C, const double* Qn, const double* Rn, const double* x0, const double* P0,
+                       bmpc_estimator** out);
+/* P [batch,nx,nx] (full, symmetric) and status [batch] of a Kalman filter; either may be NULL.  Synchronises.  BMPC_ERR_ARG on a
+ * fixed-gain estimator. */
+int bmpc_est_get_cov(bmpc_estimator* e, double* P, int32_t* status);
+/* replace any of the matrices of a created estimator between steps (time-varying model); NULL keeps an array.  L applies to the
+ * fixed-gain estimator only, Qn and Rn to the Kalman filter only: the wrong kind returns BMPC_ERR_ARG.  Layout and leading n_sys
+ * dimension as at creation; on_device = 0: host pointers, 1: device pointers on the estimator's device.  Stream-ordered on the
+ * estimator's stream (the controller's once attached): whatever wrote device arrays must be ordered before it, and they stay
+ * unchanged until that stream has passed this call.  A, B and Qn act from the next predict, C and Rn (and L) from the next update;
+ * y is not recomputed. */
+int bmpc_est_set_model(bmpc_estimator* e, const double* A, const double* B, const double* C, const double* L, const double* Qn,
+                       const double* Rn, int on_device);
+
 /* ---- batched DARE, the design step of kalman_design / kalman_design_simple (kalman.py:67, 96: control.dare):
  *   X = A'XA - (A'XB + S)(R + B'XB)^-1 (B'XA + S') + Q,   G = (R + B'XB)^-1 (B'XA + S')
  * for `batch` independent instances, 1 <= n, m <= 32, by structured doubling in fp64 (csrc/bmpc_dare.cuh).

@@ -32,7 +32,8 @@ EXPORTS = ["bmpc_default_config", "bmpc_create", "bmpc_destroy", "bmpc_last_erro
            "bmpc_gather_arrive", "bmpc_set_stream",
            "bmpc_synchronize", "bmpc_get_stats", "bmpc_get_sys", "bmpc_get_dims", "bmpc_host_alloc",
            "bmpc_host_free", "bmpc_device_count", "bmpc_has_fast_path", "bmpc_has_multi_input_fast_path", "bmpc_est_create", "bmpc_est_create_ex", "bmpc_est_destroy", "bmpc_est_predict",
-           "bmpc_est_update", "bmpc_est_get", "bmpc_est_state_ptr", "bmpc_est_set_stream", "bmpc_est_attach", "bmpc_dare"]
+           "bmpc_est_update", "bmpc_est_get", "bmpc_est_state_ptr", "bmpc_est_set_stream", "bmpc_est_attach", "bmpc_est_create_kf",
+           "bmpc_est_get_cov", "bmpc_est_set_model", "bmpc_dare"]
 
 
 class BmpcError(RuntimeError):
@@ -85,6 +86,9 @@ def load(path=None):
     L.bmpc_est_state_ptr.argtypes = [P]; L.bmpc_est_state_ptr.restype = P
     L.bmpc_est_set_stream.argtypes = [P, P]; L.bmpc_est_set_stream.restype = ctypes.c_int
     L.bmpc_est_attach.argtypes = [P, P]; L.bmpc_est_attach.restype = ctypes.c_int
+    L.bmpc_est_create_kf.argtypes = [ctypes.c_int32] * 6 + [DP] * 7 + [ctypes.POINTER(P)]; L.bmpc_est_create_kf.restype = ctypes.c_int
+    L.bmpc_est_get_cov.argtypes = [P, DP, DP]; L.bmpc_est_get_cov.restype = ctypes.c_int
+    L.bmpc_est_set_model.argtypes = [P] + [DP] * 6 + [ctypes.c_int]; L.bmpc_est_set_model.restype = ctypes.c_int
     L.bmpc_dare.argtypes = [ctypes.c_int32] * 4 + [DP] * 9; L.bmpc_dare.restype = ctypes.c_int
     L.bmpc_has_fast_path.argtypes = [ctypes.c_int] * 4; L.bmpc_has_fast_path.restype = ctypes.c_int
     L.bmpc_has_multi_input_fast_path.argtypes = [ctypes.c_int] * 4; L.bmpc_has_multi_input_fast_path.restype = ctypes.c_int

@@ -25,6 +25,7 @@
 #include "bmpc_launch.cuh"
 #include "bmpc_tpm.cuh"
 #include "bmpc_dare.cuh"
+#include "bmpc_kf.cuh"
 
 // One block of round counters = BMPC_CNT ints (the handle keeps two, used alternately): [0] instances still unfinished (-> next list),
 // [1] active-set refinements, [2] overflow of the small polish tier, [3] certified infeasible, [4..7] queue control of k_tpi_pol
@@ -2230,9 +2231,42 @@ __global__ void k_dare(int n, int m, int batch, const double* __restrict__ A, co
     if (t.tid == 0) { status[b] = st; steps[b] = it; }
 }
 
+// batched Kalman filter (csrc/bmpc_kf.cuh): one thread per instance; P and the intermediates field-major in global memory.
+// k_kf: one shared model, held in shared memory
+__global__ void k_kf(int nx, int nu, int ny, int B, const double* __restrict__ mats, double* __restrict__ x, double* __restrict__ y,
+                     double* __restrict__ P, double* __restrict__ ws, int* __restrict__ status, const double* __restrict__ in, int mode) {
+    extern __shared__ double sm[];
+    const BmpcKfLayout l = bmpc_kf_layout(nx, nu, ny);
+    for (int i = threadIdx.x; i < l.model; i += blockDim.x) sm[i] = mats[i];
+    __syncthreads();
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= B) return;
+    bmpc_kf_step(BmpcKfModel<false>{sm, 1, nx, nu, ny, l}, b, B, mode, in, x, y, P, ws, status);
+}
+
+// k_kf_pi: one model per instance, field-major in global memory (element e of instance b at mats[e * B + b])
+__global__ void k_kf_pi(int nx, int nu, int ny, int B, const double* __restrict__ mats, double* __restrict__ x, double* __restrict__ y,
+                        double* __restrict__ P, double* __restrict__ ws, int* __restrict__ status, const double* __restrict__ in, int mode) {
+    const BmpcKfLayout l = bmpc_kf_layout(nx, nu, ny);
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= B) return;
+    bmpc_kf_step(BmpcKfModel<true>{mats + b, (size_t)B, nx, nu, ny, l}, b, B, mode, in, x, y, P, ws, status);
+}
+
+// bmpc_est_set_model of per-instance arrays: src [n, cnt] batch-major -> dst field-major (element k of instance s at dst[k * n + s])
+__global__ void k_est_put(const double* __restrict__ src, int cnt, int n, double* __restrict__ dst) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (size_t)cnt * n) return;
+    const size_t k = i / n, s = i % n;
+    dst[i] = src[s * cnt + k];
+}
+
 struct bmpc_estimator {
     int nx, nu, ny, B, device, n_sys;
+    int kf = 0;                        // 0: fixed gain L (k_est, k_est_pi); 1: Kalman filter (k_kf, k_kf_pi)
     double *mats = nullptr, *x = nullptr, *y = nullptr, *in = nullptr;
+    double *P = nullptr, *ws = nullptr, *stage = nullptr;   // Kalman filter: packed P and workspace (field-major); set_model staging
+    int* status = nullptr;
     cudaStream_t stream = nullptr, own = nullptr;
     bmpc_handle* mpc = nullptr;        // attached controller: same stream, and its deferred solve is retired before its u0 is read
 };
@@ -2244,6 +2278,62 @@ int bmpc_est_create(int32_t nx, int32_t nu, int32_t ny, int32_t batch, int32_t d
     return bmpc_est_create_ex(nx, nu, ny, batch, 1, device, A, B, C, L, x0, out);
 }
 
+// the model's fields in the order of e->mats: fixed gain (A, B, C, L); Kalman filter (A, B, C, Qn, Rn), bmpc_kf_layout's order
+static int est_fields(const bmpc_estimator* e, size_t* cnt) {
+    const size_t nx = e->nx, nu = e->nu, ny = e->ny;
+    cnt[0] = nx * nx; cnt[1] = nx * nu; cnt[2] = ny * nx;
+    if (!e->kf) { cnt[3] = nx * ny; return 4; }
+    cnt[3] = nx * nx; cnt[4] = ny * ny; return 5;
+}
+
+// allocate and upload a new estimator's state: the model's fields (src, in est_fields' order), x0, y = C x0 and, for the Kalman
+// filter, P0 and the status.  On failure the caller destroys e.
+static int est_init(bmpc_estimator* e, const double* const* src, const double* x0, const double* P0) {
+    const int nx = e->nx, ny = e->ny, batch = e->B, n_sys = e->n_sys;
+    size_t cnt[5]; const int nf = est_fields(e, cnt);
+    size_t nm = 0; for (int f = 0; f < nf; f++) nm += cnt[f];
+    const int mx = e->nu > ny ? e->nu : ny;
+    bool ok = cudaMalloc((void**)&e->mats, nm * n_sys * 8) == cudaSuccess && cudaMalloc((void**)&e->x, (size_t)batch * nx * 8) == cudaSuccess &&
+              cudaMalloc((void**)&e->y, (size_t)batch * ny * 8) == cudaSuccess && cudaMalloc((void**)&e->in, (size_t)batch * mx * 8) == cudaSuccess &&
+              cudaStreamCreateWithFlags(&e->own, cudaStreamNonBlocking) == cudaSuccess;
+    const BmpcKfLayout l = bmpc_kf_layout(nx, e->nu, ny);
+    if (ok && e->kf)
+        ok = cudaMalloc((void**)&e->P, (size_t)l.P * batch * 8) == cudaSuccess && cudaMalloc((void**)&e->ws, (size_t)l.ws * batch * 8) == cudaSuccess &&
+             cudaMalloc((void**)&e->status, (size_t)batch * 4) == cudaSuccess;
+    if (!ok) { g_create_err = "bmpc_est_create: allocation failed"; return BMPC_ERR_CUDA; }
+    e->stream = e->own;
+    // packed fields of each system; with n_sys = batch transposed to field-major for k_est_pi / k_kf_pi
+    std::vector<double> m(nm * n_sys);
+    for (int s = 0; s < n_sys; s++) {
+        size_t e0 = 0;
+        for (int f = 0; f < nf; f++) {
+            for (size_t k = 0; k < cnt[f]; k++) m[(e0 + k) * n_sys + s] = src[f][s * cnt[f] + k];
+            e0 += cnt[f];
+        }
+    }
+    cudaMemcpyAsync(e->mats, m.data(), m.size() * 8, cudaMemcpyHostToDevice, e->stream);
+    cudaMemcpyAsync(e->x, x0, (size_t)batch * nx * 8, cudaMemcpyHostToDevice, e->stream);
+    // y = C x0 (kalman.py:113): a predict with A = I, B = 0 would do; compute on the host instead (setup only)
+    const double* C = src[2];
+    std::vector<double> y0((size_t)batch * ny);
+    for (int b = 0; b < batch; b++) {
+        const double* Cb = C + (n_sys == 1 ? 0 : (size_t)b * ny * nx);
+        for (int i = 0; i < ny; i++) { double acc = 0; for (int j = 0; j < nx; j++) acc += Cb[i * nx + j] * x0[(size_t)b * nx + j]; y0[(size_t)b * ny + i] = acc; }
+    }
+    cudaMemcpyAsync(e->y, y0.data(), y0.size() * 8, cudaMemcpyHostToDevice, e->stream);
+    std::vector<double> Ph; std::vector<int> st;
+    if (e->kf) {                       // upper triangle of P0, packed, field-major
+        Ph.resize((size_t)l.P * batch); st.assign(batch, BMPC_KF_OK);
+        for (int b = 0; b < batch; b++)
+            for (int i = 0; i < nx; i++)
+                for (int j = i; j < nx; j++) Ph[(size_t)bmpc_kf_pk(nx, i, j) * batch + b] = P0[((size_t)b * nx + i) * nx + j];
+        cudaMemcpyAsync(e->P, Ph.data(), Ph.size() * 8, cudaMemcpyHostToDevice, e->stream);
+        cudaMemcpyAsync(e->status, st.data(), st.size() * 4, cudaMemcpyHostToDevice, e->stream);
+    }
+    if (cudaStreamSynchronize(e->stream) != cudaSuccess) { g_create_err = "bmpc_est_create: upload failed"; return BMPC_ERR_CUDA; }
+    return BMPC_OK;
+}
+
 int bmpc_est_create_ex(int32_t nx, int32_t nu, int32_t ny, int32_t batch, int32_t n_sys, int32_t device, const double* A, const double* B,
                        const double* C, const double* L, const double* x0, bmpc_estimator** out) {
     if (!out || !A || !B || !C || !L || !x0 || nx < 1 || nx > 32 || nu < 1 || ny < 1 || batch < 1) { g_create_err = "bmpc_est_create: bad argument (1 <= nx <= 32)"; return BMPC_ERR_ARG; }
@@ -2253,34 +2343,37 @@ int bmpc_est_create_ex(int32_t nx, int32_t nu, int32_t ny, int32_t batch, int32_
     cudaSetDevice(device);
     bmpc_estimator* e = new bmpc_estimator();
     e->nx = nx; e->nu = nu; e->ny = ny; e->B = batch; e->device = device; e->n_sys = n_sys;
-    const size_t nm = (size_t)nx * nx + (size_t)nx * nu + (size_t)ny * nx + (size_t)nx * ny;
-    const int mx = nu > ny ? nu : ny;
-    bool ok = cudaMalloc((void**)&e->mats, nm * n_sys * 8) == cudaSuccess && cudaMalloc((void**)&e->x, (size_t)batch * nx * 8) == cudaSuccess &&
-              cudaMalloc((void**)&e->y, (size_t)batch * ny * 8) == cudaSuccess && cudaMalloc((void**)&e->in, (size_t)batch * mx * 8) == cudaSuccess &&
-              cudaStreamCreateWithFlags(&e->own, cudaStreamNonBlocking) == cudaSuccess;
-    if (!ok) { g_create_err = "bmpc_est_create: allocation failed"; bmpc_est_destroy(e); return BMPC_ERR_CUDA; }
-    e->stream = e->own;
-    // packed (A, B, C, L) of each system; with n_sys = batch transposed to field-major for k_est_pi
-    const size_t cnt[4] = {(size_t)nx * nx, (size_t)nx * nu, (size_t)ny * nx, (size_t)nx * ny};
     const double* src[4] = {A, B, C, L};
-    std::vector<double> m(nm * n_sys);
-    for (int s = 0; s < n_sys; s++) {
-        size_t e0 = 0;
-        for (int f = 0; f < 4; f++) {
-            for (size_t k = 0; k < cnt[f]; k++) m[(e0 + k) * n_sys + s] = src[f][s * cnt[f] + k];
-            e0 += cnt[f];
+    const int rc = est_init(e, src, x0, nullptr);
+    if (rc) { bmpc_est_destroy(e); return rc; }
+    *out = e;
+    return BMPC_OK;
+}
+
+int bmpc_est_create_kf(int32_t nx, int32_t nu, int32_t ny, int32_t batch, int32_t n_sys, int32_t device, const double* A,
+                       const double* B, const double* C, const double* Qn, const double* Rn, const double* x0, const double* P0,
+                       bmpc_estimator** out) {
+    if (!out || !A || !B || !C || !Qn || !Rn || !x0 || !P0 || nx < 1 || nx > BMPC_KF_MAX_DIM || nu < 1 || ny < 1 || ny > BMPC_KF_MAX_DIM || batch < 1) {
+        g_create_err = "bmpc_est_create_kf: bad argument (1 <= nx, ny <= 32, nu >= 1)"; return BMPC_ERR_ARG;
+    }
+    if (n_sys != 1 && n_sys != batch) { g_create_err = "bmpc_est_create_kf: n_sys must be 1 (shared model) or batch (one model per instance)"; return BMPC_ERR_ARG; }
+    *out = nullptr;
+    if (device < 0 || bmpc_device_count() <= device) { g_create_err = "no CUDA device visible: libbmpc has no CPU fallback"; return BMPC_ERR_NO_DEVICE; }
+    cudaSetDevice(device);
+    const size_t smem = (size_t)bmpc_kf_layout(nx, nu, ny).model * 8;
+    if (n_sys == 1 && smem > 48 * 1024) {              // the shared model of k_kf: large nu needs the opt-in shared memory
+        int optin = 0;
+        cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device);
+        if (smem > (size_t)optin) { g_create_err = "bmpc_est_create_kf: the shared model exceeds the shared memory of one block (use n_sys = batch)"; return BMPC_ERR_ARG; }
+        if (cudaFuncSetAttribute(k_kf, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
+            g_create_err = "bmpc_est_create_kf: cannot raise the dynamic shared memory limit"; return BMPC_ERR_CUDA;
         }
     }
-    cudaMemcpyAsync(e->mats, m.data(), m.size() * 8, cudaMemcpyHostToDevice, e->stream);
-    cudaMemcpyAsync(e->x, x0, (size_t)batch * nx * 8, cudaMemcpyHostToDevice, e->stream);
-    // y = C x0 (kalman.py:113): a predict with A = I, B = 0 would do; compute on the host instead (setup only)
-    std::vector<double> y0((size_t)batch * ny);
-    for (int b = 0; b < batch; b++) {
-        const double* Cb = C + (n_sys == 1 ? 0 : (size_t)b * ny * nx);
-        for (int i = 0; i < ny; i++) { double acc = 0; for (int j = 0; j < nx; j++) acc += Cb[i * nx + j] * x0[(size_t)b * nx + j]; y0[(size_t)b * ny + i] = acc; }
-    }
-    cudaMemcpyAsync(e->y, y0.data(), y0.size() * 8, cudaMemcpyHostToDevice, e->stream);
-    if (cudaStreamSynchronize(e->stream) != cudaSuccess) { g_create_err = "bmpc_est_create: upload failed"; bmpc_est_destroy(e); return BMPC_ERR_CUDA; }
+    bmpc_estimator* e = new bmpc_estimator();
+    e->nx = nx; e->nu = nu; e->ny = ny; e->B = batch; e->device = device; e->n_sys = n_sys; e->kf = 1;
+    const double* src[5] = {A, B, C, Qn, Rn};
+    const int rc = est_init(e, src, x0, P0);
+    if (rc) { bmpc_est_destroy(e); return rc; }
     *out = e;
     return BMPC_OK;
 }
@@ -2288,7 +2381,7 @@ int bmpc_est_create_ex(int32_t nx, int32_t nu, int32_t ny, int32_t batch, int32_
 void bmpc_est_destroy(bmpc_estimator* e) {
     if (!e) return;
     cudaSetDevice(e->device);
-    cudaFree(e->mats); cudaFree(e->x); cudaFree(e->y); cudaFree(e->in);
+    cudaFree(e->mats); cudaFree(e->x); cudaFree(e->y); cudaFree(e->in); cudaFree(e->P); cudaFree(e->ws); cudaFree(e->stage); cudaFree(e->status);
     if (e->own) cudaStreamDestroy(e->own);
     delete e;
 }
@@ -2306,6 +2399,14 @@ static int est_run(bmpc_estimator* e, const double* in, int n, int on_device, in
     if (!on_device) {
         if (cudaMemcpyAsync(e->in, in, (size_t)e->B * n * 8, cudaMemcpyHostToDevice, e->stream) != cudaSuccess) return BMPC_ERR_CUDA;
         src = e->in;
+    }
+    if (e->kf) {
+        const BmpcKfLayout l = bmpc_kf_layout(e->nx, e->nu, e->ny);
+        if (e->n_sys == 1)
+            k_kf<<<(e->B + 127) / 128, 128, (size_t)l.model * 8, e->stream>>>(e->nx, e->nu, e->ny, e->B, e->mats, e->x, e->y, e->P, e->ws, e->status, src, mode);
+        else
+            k_kf_pi<<<(e->B + 127) / 128, 128, 0, e->stream>>>(e->nx, e->nu, e->ny, e->B, e->mats, e->x, e->y, e->P, e->ws, e->status, src, mode);
+        return cudaGetLastError() == cudaSuccess ? BMPC_OK : BMPC_ERR_CUDA;
     }
     const size_t nm = (size_t)e->nx * e->nx + (size_t)e->nx * e->nu + (size_t)e->ny * e->nx + (size_t)e->nx * e->ny;
     if (e->n_sys == 1)
@@ -2330,6 +2431,53 @@ int bmpc_est_attach(bmpc_estimator* e, bmpc_handle* h) {
     if (h && h->cfg.device != e->device) return BMPC_ERR_ARG;
     cudaSetDevice(e->device); cudaStreamSynchronize(e->stream);
     e->mpc = h; e->stream = h ? h->stream : e->own;
+    return BMPC_OK;
+}
+
+int bmpc_est_get_cov(bmpc_estimator* e, double* P, int32_t* status) {
+    if (!e || !e->kf) return BMPC_ERR_ARG;
+    cudaSetDevice(e->device);
+    const int nx = e->nx, B = e->B;
+    std::vector<double> Ph;
+    if (P) { Ph.resize((size_t)bmpc_kf_layout(nx, e->nu, e->ny).P * B); cudaMemcpyAsync(Ph.data(), e->P, Ph.size() * 8, cudaMemcpyDeviceToHost, e->stream); }
+    if (status) cudaMemcpyAsync(status, e->status, (size_t)B * 4, cudaMemcpyDeviceToHost, e->stream);
+    if (cudaStreamSynchronize(e->stream) != cudaSuccess) return BMPC_ERR_CUDA;
+    if (P)
+        for (int b = 0; b < B; b++)
+            for (int i = 0; i < nx; i++)
+                for (int j = 0; j < nx; j++) P[((size_t)b * nx + i) * nx + j] = Ph[(size_t)bmpc_kf_pk(nx, i, j) * B + b];
+    return BMPC_OK;
+}
+
+int bmpc_est_set_model(bmpc_estimator* e, const double* A, const double* B, const double* C, const double* L, const double* Qn,
+                       const double* Rn, int on_device) {
+    if (!e || (e->kf ? L != nullptr : (Qn != nullptr || Rn != nullptr))) return BMPC_ERR_ARG;
+    if (cudaSetDevice(e->device) != cudaSuccess) return BMPC_ERR_CUDA;
+    if (e->mpc) e->stream = e->mpc->stream;
+    size_t cnt[5]; const int nf = est_fields(e, cnt);
+    const double* kf_src[5] = {A, B, C, Qn, Rn};
+    const double* est_src[4] = {A, B, C, L};
+    const double* const* src = e->kf ? kf_src : est_src;
+    size_t nm = 0; for (int f = 0; f < nf; f++) nm += cnt[f];
+    const size_t n = e->n_sys;
+    const cudaMemcpyKind kind = on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+    size_t off = 0;
+    for (int f = 0; f < nf; off += cnt[f], f++) {
+        if (!src[f]) continue;
+        if (n == 1) {                                     // packed: the array is the field
+            if (cudaMemcpyAsync(e->mats + off, src[f], cnt[f] * 8, kind, e->stream) != cudaSuccess) return BMPC_ERR_CUDA;
+            continue;
+        }
+        const double* d = src[f];
+        if (!on_device) {                                 // host arrays go through a staging copy, one region per field
+            if (!e->stage && cudaMalloc((void**)&e->stage, nm * n * 8) != cudaSuccess) return BMPC_ERR_CUDA;
+            if (cudaMemcpyAsync(e->stage + off * n, src[f], cnt[f] * n * 8, kind, e->stream) != cudaSuccess) return BMPC_ERR_CUDA;
+            d = e->stage + off * n;
+        }
+        const size_t tot = cnt[f] * n;
+        k_est_put<<<(unsigned)((tot + 255) / 256), 256, 0, e->stream>>>(d, (int)cnt[f], (int)n, e->mats + off * n);
+        if (cudaGetLastError() != cudaSuccess) return BMPC_ERR_CUDA;
+    }
     return BMPC_OK;
 }
 
